@@ -1,9 +1,9 @@
 """`bench.py --impl reference`: drive the UNMODIFIED reference (pip --target baseline/_ref) on the headline
 config through its own public API and stock code path -- its `train_config`, `get_model_config`,
 `get_policies`, `get_dummy_loader`, torch FSDP wrap exactly as its `main_training_llama.py:82-115`, its
-`train()` loop (torch.compile as in its defaults).  None of the B200 engine is imported.
+`train()` loop (torch.compile as in its defaults).  None of this repository's engine is imported.
 
-Outcome of the offline install (also recorded in DESIGN.md): `pip install --no-index ... /root/reference` fails
+Outcome of the offline install (also recorded in DESIGN.md): `pip install --no-index ... <reference checkout>` fails
 on the missing `ibm-fms` requirement; `--no-deps` installs `fms_fsdp` + `speculator`.  `ibm-fms` and `fire` cannot
 be installed (no index), so `baseline/fms_shim/` provides plain-PyTorch stand-ins for the handful of fms classes
 the reference imports.  Timing: the K timed steps are ONE call of the reference's `train()` (which moves each

@@ -1,8 +1,11 @@
 #!/usr/bin/env python
-"""Headline benchmark: tokens/sec for Llama2-7B FSDP, seq 4096, per-GPU batch 2, bf16, synthetic data
-(BASELINE.json; the reference's `use_dummy_dataset` stream, reference dataloader_utils.py:36-57).
+"""Headline benchmark: tokens/sec for Llama FSDP, seq 4096, per-GPU batch 2, bf16, synthetic data
+(the reference's `use_dummy_dataset` stream, reference dataloader_utils.py:36-57).  The default model is Llama2-7B
+wherever its memory plan fits the 80 GB per GPU (4 or more H100s); with fewer GPUs it is Llama2-1.4B, because 7B's
+unsharded fp32 master weights, AdamW state and activations take ~133 GiB.
 
     python bench.py --gpus 1 --steps 10 --warmup 3
+    python bench.py --gpus 1 --steps 10 --warmup 3 --dump-outputs /tmp/out    # also write the last step's outputs
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus 8 --steps 10 --warmup 3
     python bench.py --impl reference ...      # the unmodified reference from baseline/_ref
@@ -26,6 +29,8 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
+HEADLINE_MODEL, SMALL_MODEL = "llama2_7b", "llama2_1.4b"
+DUMP_PARAM_SAMPLE = 4 * 2**20      # fp32 master-weight elements written by --dump-outputs (16 MB)
 BASELINE_TOK_S_GPU = 9600.0  # BASELINE.md: Llama2-7B on 96x H100, reference README.md:16 (best published)
 # best published tokens/s/GPU per model (BASELINE.md section 1, H100 column); models without a published number -> null
 PUBLISHED_TOK_S_GPU = {"llama2_7b": 9600.0, "llama2_13b": 4850.0, "llama2_34b": 1830.0, "llama2_70b": 890.0}
@@ -37,7 +42,8 @@ def _args():
     p.add_argument("--steps", type=int, default=8)
     p.add_argument("--warmup", type=int, default=3)
     p.add_argument("--impl", default="ours", choices=["ours", "reference"])
-    p.add_argument("--model", default="llama2_7b")
+    p.add_argument("--model", default=None,
+                   help="default: Llama2-7B where its memory plan fits the GPUs (8 x 80 GB), else Llama2-1.4B")
     p.add_argument("--seq", type=int, default=4096)
     p.add_argument("--batch", type=int, default=2)
     p.add_argument("--sharding", default="fsdp")
@@ -49,7 +55,20 @@ def _args():
     p.add_argument("--nlayers", type=int, default=0, help="debug only: override depth (result is flagged invalid)")
     p.add_argument("--trace", default="", help="with --profile: also export the chrome trace of the 2 profiled steps")
     p.add_argument("--profile", default="", help="write a per-kernel device-time table of 2 extra steps to this path")
-    return p.parse_args()
+    p.add_argument("--dump-outputs", default="", metavar="DIR",
+                   help="after the timed steps, write what the last timed step computed (loss, grad norm, a fixed "
+                        "sample of the updated fp32 master weights) as DIR/<name>.npy")
+    a = p.parse_args()
+    if a.model is None:
+        a.model = default_model(a.gpus)
+    return a
+
+
+def default_model(gpus):
+    """The headline Llama2-7B wherever its per-GPU memory plan fits (batch 2, seq 4096, no recomputation), the 1.4B model
+    of the same family on fewer GPUs (7B unsharded needs ~133 GiB)."""
+    from fms_fsdp_b200.utils.memory_plan import plan_llama
+    return HEADLINE_MODEL if plan_llama(HEADLINE_MODEL, gpus=gpus).fits() else SMALL_MODEL
 
 
 DATA_NOTE = "synthetic (reference get_dummy_loader stream, random-init weights)"
@@ -59,11 +78,11 @@ def bench_config(model, global_batch, seq, parallelism, ac):
     """The SAME keys (and, for the same run, values) in both arms."""
     return {"model": model, "global_batch": global_batch, "seq_len": seq, "parallelism": parallelism,
             "selective_ac": str(ac), "data_stream": "get_dummy_loader (arange windows mod vocab, label == input)",
-            "l2": "per-step working set (>=13.5 GB of weights+activations) >> 126 MB L2; no explicit flush"}
+            "l2": "per-step working set (GBs of weights+activations) >> 50 MB L2; no explicit flush"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -232,6 +251,8 @@ def run_ours(a):
     launches = CK.launch_count()
     fallbacks = CK.fallback_count()
     peak_alloc = torch.cuda.max_memory_allocated(dev)   # train() below resets the peak counters at its report step
+    if a.dump_outputs:     # after the peak is read: gathering whole fp32 units for the sample is not part of a step
+        dump_outputs(a.dump_outputs, eng, loss, gn, rank)
     loss_timed = float(loss_sum) / a.steps      # mean loss of steps W+1 .. W+K (what the reference arm prints too)
     ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
     if world > 1:
@@ -265,7 +286,7 @@ def run_ours(a):
            "ddp": f"ddp{world}"}.get(a.sharding, a.sharding)
     if rank == 0:
         out = {
-            "metric": "tokens/sec (Llama2-7B FSDP seq4k bs2)" if a.model == "llama2_7b" else f"tokens/sec ({a.model})",
+            "metric": f"tokens/sec ({a.model} FSDP seq{a.seq} bs{a.batch})",
             "value": round(value, 1), "unit": "tokens/s",
             "n_gpus": world, "steps": a.steps, "warmup": a.warmup, "ms_per_step": round(ms_step, 3),
             "higher_is_better": True, "scaling": "weak",
@@ -298,7 +319,7 @@ def run_ours(a):
             out["invalid"] = "reduced-precision run (opt-in fp8 forward GEMMs): not the headline metric"
         if fallbacks:
             out["invalid"] = f"{fallbacks} ops of the timed region ran on the ATen fallback: {dict(CK.FALLBACKS)}"
-        if a.model != "llama2_7b" or a.seq != 4096 or a.batch != 2:
+        if a.model != default_model(world) or a.seq != 4096 or a.batch != 2:
             out["note"] = "secondary configuration, not the BASELINE headline"
         print(json.dumps(out), flush=True)
     if a.profile:
@@ -319,6 +340,30 @@ def run_ours(a):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, eng, loss, grad_norm, rank):
+    """The last timed step's results as float32 .npy files: the loss and grad norm it returned, and a fixed sample of the
+    fp32 master weights its optimizer step produced (every unit, evenly strided so two builds sample the same
+    elements).  Collective over ranks (the master weights are gathered); rank 0 writes."""
+    import numpy as np
+    import torch
+
+    total = sum(u.layout.total for u in eng.units)
+    parts = []
+    for u in eng.units:
+        full = eng.gather_unit_full(u, "master").reshape(-1)
+        n = full.numel()
+        k = min(n, max(1, DUMP_PARAM_SAMPLE * u.layout.total // total))
+        idx = torch.div(torch.arange(k, device=full.device, dtype=torch.int64) * n, k, rounding_mode="floor")
+        parts.append(full[idx].float().cpu())
+        del full
+    if rank != 0:
+        return
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.asarray([float(loss)], dtype=np.float32))
+    np.save(os.path.join(out_dir, "grad_norm.npy"), np.asarray([float(grad_norm)], dtype=np.float32))
+    np.save(os.path.join(out_dir, "master_weights_sample.npy"), torch.cat(parts).numpy().astype(np.float32))
 
 
 def run_reference(a):

@@ -1,4 +1,4 @@
-"""Compatibility alias: ``fms_fsdp.*`` resolves to the B200-native implementation ``fms_fsdp_b200.*`` so
+"""Compatibility alias: ``fms_fsdp.*`` resolves to the H100-native implementation ``fms_fsdp_b200.*`` so
 code written against the reference's public API (``from fms_fsdp.config import train_config``,
 ``from fms_fsdp.policies import ...``, ``from fms_fsdp.utils.train_utils import train`` ...) runs unchanged."""
 import importlib

@@ -1,12 +1,12 @@
-"""In-tree build of the sm_100a extension ``fms_fsdp_b200/_C.so``.
+"""In-tree build of the sm_90a extension ``fms_fsdp_b200/_C.so``.
 
     python -m fms_fsdp_b200.build            # incremental
     python -m fms_fsdp_b200.build --force
 
-* every ``csrc/*.cu`` is torch-free and compiled by nvcc for ``compute_100a/sm_100a`` with ``-lineinfo``
+* every ``csrc/*.cu`` is torch-free and compiled by nvcc for ``compute_90a/sm_90a`` with ``-lineinfo``
   (ncu source pages) -- nvcc cross-compiles without a GPU;
 * ``csrc/bindings.cpp`` (torch/pybind) is compiled by g++ only;
-* the .so stays in the tree (git-ignored) so it travels to the GPU box with the snapshot.
+* the .so stays in the tree (git-ignored), next to the package, so the package imports from the source tree.
 """
 from __future__ import annotations
 
@@ -19,12 +19,12 @@ from concurrent.futures import ThreadPoolExecutor
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-BUILD = os.path.join(HERE, "..", "build", "b200_ext")
+BUILD = os.path.join(HERE, "..", "build", "sm90_ext")
 OUT = os.path.join(HERE, "_C.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("CXX", "g++")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo",
               "--use_fast_math", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
@@ -89,7 +89,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
         with ThreadPoolExecutor(max_workers=min(8, len(jobs))) as ex:
             for base in ex.map(do, jobs):
                 if verbose:
-                    print(f"[b200 build] compiled {base}", flush=True)
+                    print(f"[build] compiled {base}", flush=True)
     if jobs or force or not os.path.exists(OUT):
         tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
         cuda_lib = "/usr/local/cuda/lib64"
@@ -98,7 +98,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
             "-ltorch_python", "-lcudart", f"-Wl,-rpath,{tlib}", f"-Wl,-rpath,{cuda_lib}"]
         _run(cmd, os.path.join(BUILD, "link.log"))
         if verbose:
-            print(f"[b200 build] linked {OUT}", flush=True)
+            print(f"[build] linked {OUT}", flush=True)
     return OUT
 
 

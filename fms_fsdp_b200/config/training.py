@@ -3,7 +3,7 @@
 One flat dataclass; every field is a ``--field=value`` CLI flag of the entry
 points (parity with the reference's ``fms_fsdp/config/training.py:5-74``).
 Field names and defaults follow the reference so existing launch scripts keep
-working; the block at the bottom holds the B200-specific extension knobs
+working; the block at the bottom holds the engine-specific extension knobs
 (SURVEY.md App. B "new knobs"), whose defaults preserve reference behaviour.
 """
 from dataclasses import dataclass, field
@@ -94,11 +94,11 @@ class train_config:
     stage2_batch_size: int = 96                       # speculator stage 2: generation batch
     stage2_seq_length: int = 256                      # speculator stage 2: generated tokens per prompt
 
-    # ---- B200 engine extensions (not in the reference; defaults keep reference semantics)
+    # ---- engine extensions (not in the reference; defaults keep reference semantics)
     comm_backend: str = "auto"               # auto | nccl | gloo
     collective_impl: str = "auto"            # auto | fused (NVLink peer kernels) | torch (c10d collectives)
     hsdp_shard_size: int = 0                 # 0 = local device count (reference behaviour); 4 -> 2x4 on one box
-    kernel_path: str = "auto"                # auto | fused (sm_100a kernels) | torch (ATen oracle)
+    kernel_path: str = "auto"                # auto | fused (sm_90a kernels) | torch (ATen oracle)
     precision: str = "bf16"                  # bf16 | fp8 (opt-in: row-wise scaled e4m3 forward GEMMs, bf16 backward)
     prefetch_depth: int = 2                  # gathered-unit buffers in flight (reference limiter = 2)
     fused_cross_entropy: bool = True         # linear+CE without materialising logits

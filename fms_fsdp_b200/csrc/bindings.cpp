@@ -40,7 +40,6 @@ DECL int b200_selscan_bwd(const void*, const void*, const void*, const float*, c
                           int, int, int, int, cudaStream_t);
 DECL void b200_comm_set_reduce_ctas(int);
 DECL int b200_p2p_gather_range(const void* const*, void*, long long, long long, long long, cudaStream_t);
-DECL int b200_ts_mma_probe(const void*, const void*, float*, cudaStream_t);
 DECL int b200_rmsnorm_fwd(const void*, const void*, void*, float*, int, int, float, cudaStream_t);
 DECL int b200_rmsnorm_bwd_grid(int);
 DECL int b200_rmsnorm_bwd(const void*, const void*, const void*, const float*, const void*, void*, float*, float*, int, int,
@@ -59,9 +58,6 @@ DECL int b200_ce_grad_inplace(void*, const long long*, const float*, float*, int
 DECL int b200_adamw(float*, const void*, int, float*, float*, void*, long long, float, float, float, float, float,
                     float, float, const float*, cudaStream_t);
 DECL int b200_sumsq(const void*, int, long long, float*, cudaStream_t);
-DECL void b200_attn_set_fwd_version(int);
-DECL void b200_attn_set_bwd_version(int);
-DECL void b200_attn_set_poly(int, int);
 DECL int b200_attn_fwd(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t);
 DECL int b200_attn_bwd(const void*, const void*, const void*, const float*, void*, float*, int, int, int, int, int,
                        float, const float*, cudaStream_t);
@@ -85,7 +81,7 @@ DECL int b200_causal_conv1d_bwd(const void*, const void*, const void*, const voi
 namespace {
 
 static int64_t g_launches = 0;
-static int g_reduce_ctas_default = 296;
+static int g_reduce_ctas_default = 264;  // 2 CTAs per SM of an H100
 static bool g_gemm_2cta = true;
 
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
@@ -129,7 +125,7 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layou
   TORCH_CHECK(c.size(0) == M && c.size(1) == (epi == 6 ? 2 * N : N), "c shape mismatch");
   TORCH_CHECK(K % 8 == 0 && N % 8 == 0 && M % 8 == 0, "M, N, K must be multiples of 8");
   TORCH_CHECK((epi != 5 && epi != 6) || (g_gemm_2cta && M >= 256 && c.scalar_type() == at::kBFloat16),
-              "SwiGLU epilogues: CTA-pair kernel, bf16 output (call set_gemm_swiglu first)");
+              "SwiGLU epilogues: M >= 256, bf16 output (call set_gemm_swiglu first)");
   const void* r = nullptr;
   int ldr = 0;
   if (epi == 1) {
@@ -140,18 +136,18 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layou
     ldr = residual->stride(0);
   }
   TORCH_CHECK(epi != 3 || (g_gemm_2cta && M >= 256 && layout == 0 && c.scalar_type() == at::kBFloat16),
-              "RoPE epilogue: CTA-pair kernel, nt layout, bf16 output only (call set_gemm_rope first)");
+              "RoPE epilogue: M >= 256, nt layout, bf16 output only (call set_gemm_rope first)");
   TORCH_CHECK(epi != 4, "push epilogue: use gemm_push (no output tensor)");
-  // CTA-pair kernel (cta_group::2, 256x256 tiles) for anything with at least one full pair tile of rows
+  // fused-epilogue entry for anything with at least 256 rows; the store / residual / accumulate entry otherwise
   if (g_gemm_2cta && M >= 256) {
     check(b200_gemm2_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0),
                           ldr, a_mn, b_mn, (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()),
-          "gemm2_bf16_tcgen05");
+          "gemm2_bf16_wgmma");
     return;
   }
   check(b200_gemm_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0),
                        ldr, a_mn, b_mn, (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()),
-        "gemm_bf16_tcgen05");
+        "gemm_bf16_wgmma");
 }
 
 std::vector<at::Tensor> rmsnorm_fwd(const at::Tensor& x, const at::Tensor& w, double eps) {
@@ -446,8 +442,6 @@ std::vector<at::Tensor> causal_conv1d_bwd(const at::Tensor& dy, const at::Tensor
   return {dx, dw, db};
 }
 
-void set_attn_fwd_version(int64_t v) { b200_attn_set_fwd_version((int)v); }
-void set_attn_bwd_version(int64_t v) { b200_attn_set_bwd_version((int)v); }
 void set_gemm_2cta(bool on) { g_gemm_2cta = on; }
 bool get_gemm_2cta() { return g_gemm_2cta; }
 // GEMM with the all-gather of a unit's parameters fused in (comm warps over NVLink peer memory)
@@ -469,7 +463,7 @@ void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::T
                              (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(), (unsigned long long)shard_bytes,
                              (unsigned long long)begin, (unsigned long long)end, (int)world, (int)rank,
                              (uint32_t*)flags.data_ptr(), (uint32_t)epoch, dependent ? 1 : 0, cur_stream()),
-          "gemm2_ag_push_bf16_tcgen05");
+          "gemm2_ag_push_bf16_wgmma");
     return;
   }
   TORCH_CHECK(c_opt.has_value(), "gemm_ag: output tensor required");
@@ -493,7 +487,7 @@ void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::T
                            a_mn, b_mn, (int)epi, (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(),
                            (unsigned long long)shard_bytes, (unsigned long long)begin, (unsigned long long)end, (int)world,
                            (int)rank, (uint32_t*)flags.data_ptr(), (uint32_t)epoch, dependent ? 1 : 0, cur_stream()),
-        "gemm2_ag_bf16_tcgen05");
+        "gemm2_ag_bf16_wgmma");
 }
 // wgrad GEMM (tn: dW[M,N] = a[K,M]^T b[K,N]) whose epilogue pushes every tile to the owning rank's staging slot
 void gemm_push(const at::Tensor& a, const at::Tensor& b) {
@@ -504,9 +498,9 @@ void gemm_push(const at::Tensor& a, const at::Tensor& b) {
   need_rowmajor2d(b, "b");
   const int K = a.size(0), M = a.size(1), N = b.size(1);
   TORCH_CHECK(b.size(0) == K && g_gemm_2cta && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0,
-              "push epilogue: CTA-pair kernel (M >= 256), dims multiples of 8");
+              "push epilogue: M >= 256, dims multiples of 8");
   check(b200_gemm2_bf16(a.data_ptr(), b.data_ptr(), nullptr, nullptr, M, N, K, a.stride(0), b.stride(0), N, 0, 1, 1, 4, 0,
-                        cur_stream()), "gemm2_push_bf16_tcgen05");
+                        cur_stream()), "gemm2_push_bf16_wgmma");
 }
 // optional fp8 forward path: row-wise e4m3 quantisation and the e4m3 x e4m3 -> bf16 GEMM (kind::f8f6f4)
 std::vector<at::Tensor> quant_rowwise_e4m3(const at::Tensor& x) {
@@ -529,7 +523,7 @@ void gemm_fp8(const at::Tensor& aq, const at::Tensor& bq, const at::Tensor& sa, 
   TORCH_CHECK(bq.size(1) == K && c.size(0) == M && c.size(1) == N && sa.numel() == M && sb.numel() == N &&
               sa.is_contiguous() && sb.is_contiguous(), "gemm_fp8: shape mismatch");
   check(b200_gemm2_fp8(aq.data_ptr(), bq.data_ptr(), c.data_ptr(), sa.data_ptr<float>(), sb.data_ptr<float>(), M, N, K,
-                       (int)aq.stride(0), (int)bq.stride(0), (int)c.stride(0), cur_stream()), "gemm2_fp8_tcgen05");
+                       (int)aq.stride(0), (int)bq.stride(0), (int)c.stride(0), cur_stream()), "gemm2_fp8_wgmma");
 }
 void p2p_gather_range(const at::Tensor& peer_ptrs, at::Tensor& full, int64_t shard_bytes, int64_t begin, int64_t end) {
   c10::cuda::CUDAGuard guard(full.device());
@@ -537,15 +531,6 @@ void p2p_gather_range(const at::Tensor& peer_ptrs, at::Tensor& full, int64_t sha
         "p2p_gather_range");
 }
 
-at::Tensor ts_mma_probe(const at::Tensor& a, const at::Tensor& b) {
-  c10::cuda::CUDAGuard guard(a.device());
-  need(a, "a", at::kBFloat16);
-  need(b, "b", at::kBFloat16);
-  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && a.size(0) == 128 && a.size(1) == 64 && b.size(0) == 64 && b.size(1) == 64);
-  auto d = at::empty({128, 64}, a.options().dtype(at::kFloat));
-  check(b200_ts_mma_probe(a.data_ptr(), b.data_ptr(), d.data_ptr<float>(), cur_stream()), "ts_mma_probe");
-  return d;
-}
 int64_t launch_count() { return g_launches; }
 void reset_launch_count() { g_launches = 0; }
 
@@ -553,7 +538,7 @@ void reset_launch_count() { g_launches = 0; }
 
 
 // ------------------------------------------------------------------------------ Mamba2 SSD chunk scan (csrc/ssd.cu)
-// Orchestration of the batched tcgen05 GEMMs and the glue kernels.  Internal chunk length is 128 tokens whatever
+// Orchestration of the batched wgmma GEMMs and the glue kernels.  Internal chunk length is 128 tokens whatever
 // the model's chunk_size (the chunked form is exact for every chunking).
 namespace {
 constexpr int kL = 128;
@@ -765,7 +750,7 @@ std::vector<at::Tensor> selective_scan_bwd(const at::Tensor& dy, const at::Tenso
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "fms_fsdp_b200 sm_100a kernels";
+  m.doc() = "fms_fsdp_b200 sm_90a kernels";
   m.def("gemm", &gemm);
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd, py::arg("dy"), py::arg("x"), py::arg("w"), py::arg("rstd"), py::arg("dres") = py::none());
@@ -825,9 +810,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("selective_scan_fwd", &selective_scan_fwd);
   m.def("selective_scan_bwd", &selective_scan_bwd);
   m.def("ssd_scan_bwd", &ssd_scan_bwd);
-  m.def("set_attn_poly", [](int64_t f, int64_t b) { b200_attn_set_poly((int)f, (int)b); });
-  m.def("set_attn_fwd_version", &set_attn_fwd_version);
-  m.def("set_attn_bwd_version", &set_attn_bwd_version);
   m.def("set_gemm_2cta", &set_gemm_2cta);
   m.def("get_gemm_2cta", &get_gemm_2cta);
   m.def("gemm_ag", &gemm_ag);
@@ -835,7 +817,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("quant_rowwise_e4m3", &quant_rowwise_e4m3);
   m.def("gemm_fp8", &gemm_fp8);
   m.def("p2p_gather_range", &p2p_gather_range);
-  m.def("ts_mma_probe", &ts_mma_probe);
   m.def("launch_count", &launch_count);
   m.def("reset_launch_count", &reset_launch_count);
 }

@@ -417,7 +417,7 @@ extern "C" int b200_p2p_push_range(const void* src, void* const* bases, long lon
 // also carry the next unit's all-gather in their comm warps): a full-chip burst steals SM issue slots and NVLink
 // ingress exactly when those comm warps need it (measured at 8 GPUs: ag-GEMMs 760 -> 1080 us).  A unit's reduce only
 // has to finish within one block's backward (~5 ms), so a few dozen CTAs are enough.
-static int g_reduce_max_ctas = 148 * 2;
+static int g_reduce_max_ctas = 132 * 2;
 extern "C" void b200_comm_set_reduce_ctas(int n) { g_reduce_max_ctas = n < 1 ? 1 : n; }
 
 #define RS_CASE(BF, WW) \
@@ -451,7 +451,7 @@ extern "C" int b200_allreduce_inplace(void* const* bufs, long long numel, int wo
   long long n_slice = numel / world;
   long long nvec = n_slice / vec;
   int grid = (int)((nvec + 255) / 256);
-  if (grid > 148 * 2) grid = 148 * 2;
+  if (grid > 132 * 2) grid = 132 * 2;
   if (grid < 1) grid = 1;
   if (is_bf16) {
     switch (world) { AR_CASE(true, 1) AR_CASE(true, 2) AR_CASE(true, 4) AR_CASE(true, 8)

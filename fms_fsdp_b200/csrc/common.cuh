@@ -1,7 +1,7 @@
-// Blackwell (sm_100a) PTX building blocks shared by every kernel of the engine:
-// mbarrier pipelines, TMA bulk-tensor copies, tcgen05 (UMMA) issue/commit, TMEM alloc/load.
+// Hopper (sm_90a) PTX building blocks shared by every kernel of the engine:
+// mbarrier pipelines, TMA bulk-tensor copies, wgmma shared-memory descriptors (wgmma.cuh has the MMA wrappers).
 // Everything is inline PTX -- no CUTLASS dependency -- so the SASS shows exactly what was written
-// (UTCHMMA / LDTM / UTMALDG, see B200_PROFILING.md "What proves a Blackwell-native kernel").
+// (HGMMA / UTMALDG / SYNCS).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -100,21 +100,9 @@ B200_DEVINL void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.
 template <int N>
 B200_DEVINL void tma_store_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 
-// ------------------------------------------------------------------------------------- tcgen05
-B200_DEVINL void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-B200_DEVINL void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// whole warp; writes the TMEM base address (lane<<16 | column) to *dst_smem
-B200_DEVINL void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-B200_DEVINL void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// Shared-memory matrix descriptor, SWIZZLE_128B, descriptor version 1 (Blackwell).
+// ------------------------------------------------------------------------------------- wgmma
+// Shared-memory matrix descriptor for wgmma, SWIZZLE_128B (layout type 1 in bits 62-63), base offset 0 (tiles sit on
+// 1024 B boundaries).
 //   K-major operand : rows are 128 B (64 bf16 of K); SBO = 8 rows * 128 B = 1024; LBO unused.
 //   MN-major operand: rows are 128 B (64 bf16 of M/N) per K index; SBO = 1024 (8 K-rows),
 //                     LBO = bytes between consecutive 64-wide M/N groups (= one TMA box).
@@ -123,151 +111,12 @@ B200_DEVINL uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= 1ull << 46;  // version
-  d |= 2ull << 61;  // SWIZZLE_128B
+  d |= 1ull << 62;  // SWIZZLE_128B
   return d;
 }
 
-// Instruction descriptor for kind::f16 with bf16 inputs and fp32 accumulation.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (static_cast<uint32_t>(a_mn_major) << 15) |
-         (static_cast<uint32_t>(b_mn_major) << 16) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// Instruction descriptor for kind::f8f6f4 with e4m3 inputs (format code 0) and fp32 accumulation, both operands K-major.
-__host__ __device__ constexpr uint32_t make_idesc_e4m3(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
-
-// One lane of a CONVERGED warp.  Issue tcgen05.mma behind this instead of `lane == 0`: the compiler then knows a single
-// thread is active and emits back-to-back UTCHMMA with hoisted descriptors; a `lane == 0` branch makes it wrap every
-// UTCHMMA in an ELECT / BRA.U.ANY waterfall loop plus per-MMA descriptor rebuilds (~14 instructions per MMA, which
-// starves the tensor pipe when the issuing warp shares its scheduler with busy softmax/epilogue warps).
-B200_DEVINL bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
-
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread on behalf of the CTA.
-B200_DEVINL void umma_bf16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// A operand from TMEM (e.g. softmax probabilities written back with tcgen05.st)
-B200_DEVINL void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrive when all previously issued tcgen05 ops of this thread have completed
-B200_DEVINL void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns (thread t <-> TMEM lane base+t)
-B200_DEVINL void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-B200_DEVINL void tmem_ld_32x32b_x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-B200_DEVINL void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM (32 lanes x 16 columns of 32 bit)
-B200_DEVINL void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-B200_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-
-// ------------------------------------------------------------------- 2-CTA (cta_group::2) variants
-// A CTA pair (cluster of 2 on one TPC) runs ONE 256-row MMA: each CTA stages its 128 rows of A and its
-// half of B; the leader CTA (cluster rank 0) issues the MMA, which reads both CTAs' shared memory and
-// writes 128 accumulator lanes into each CTA's TMEM.  Halves the shared-memory traffic per FLOP.
-constexpr uint32_t kPeerBitMask = 0xFEFFFFFFu;  // clears the CTA-rank bit of a shared::cluster address
-
-B200_DEVINL uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-B200_DEVINL void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-B200_DEVINL void tmem_alloc_2cta(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-B200_DEVINL void tmem_dealloc_2cta(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load issued by either CTA of the pair; the transaction bytes are credited to the LEADER's mbarrier
-B200_DEVINL void tma_load_2d_2cta(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar) & kPeerBitMask), "r"(c0), "r"(c1)
-      : "memory");
-}
-B200_DEVINL void umma_bf16_ss_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                   uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// 8-bit operands (e4m3): K = 32 elements (= 32 bytes, the same descriptor step as bf16's K = 16) per instruction
-B200_DEVINL void umma_e4m3_ss_2cta(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                   uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f8f6f4 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on the barrier at this offset in BOTH CTAs once the issued MMAs have retired
-B200_DEVINL void umma_commit_2cta_mcast(uint64_t* bar, uint16_t cta_mask) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"(cta_mask)
-      : "memory");
-}
-// plain arrive on the LEADER CTA's copy of a barrier (callable from either CTA)
-B200_DEVINL void mbar_arrive_leader(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(smem_u32(bar) & kPeerBitMask) : "memory");
+B200_DEVINL void named_bar_sync(int id, int nthreads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 // ------------------------------------------------------------------------------------ helpers
@@ -279,20 +128,6 @@ B200_DEVINL float2 unpack_bf16x2(uint32_t u) {
   __nv_bfloat162 v = *reinterpret_cast<__nv_bfloat162*>(&u);
   return __bfloat1622float2(v);
 }
-// 2^x on the FMA pipe (Cody-Waite range reduction + degree-3 minimax polynomial, max relative error 7.5e-5; far below
-// bf16 resolution).  The MUFU unit does 16 ex2/clk/SM, which bounds flash attention at 128x128 tiles (1024 cycles per
-// tile = the tensor-pipe time of its two GEMMs); routing a fraction of the exponentials through here rebalances the
-// two pipes (same idea as FlashAttention-4's software exp).  Valid for x <= ~100; x < -126 flushes to ~2^-126.
-B200_DEVINL float exp2_poly(float x) {
-  x = fmaxf(x, -126.f);
-  const float r = x + 12582912.f;                 // 1.5 * 2^23: round-to-nearest integer lands in the low mantissa bits
-  const float f = x - (r - 12582912.f);           // in [-0.5, 0.5]
-  float p = fmaf(f, 0.055170949548482895f, 0.2426096349954605f);
-  p = fmaf(p, f, 0.6932609677314758f);
-  p = fmaf(p, f, 0.9999281764030457f);
-  return __int_as_float(__float_as_int(p) + (__float_as_int(r) << 23));   // * 2^n through the exponent field
-}
-
 B200_DEVINL float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

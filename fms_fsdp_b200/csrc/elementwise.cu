@@ -1,4 +1,4 @@
-// Bandwidth-bound kernels of the engine (sm_100a): RMSNorm fwd/bwd, RoPE, SwiGLU fwd/bwd, embedding
+// Bandwidth-bound kernels of the engine (sm_90a): RMSNorm fwd/bwd, RoPE, SwiGLU fwd/bwd, embedding
 // fwd/bwd, softmax-cross-entropy gradient (in place on a logits chunk), fused sharded AdamW, sum of
 // squares.  All are single-pass over HBM with 16-byte vector accesses; fp32 math, bf16 I/O.
 // SURVEY.md K2/K5/K7/K9/K10(softmax part)/K11/K12.
@@ -723,7 +723,7 @@ __global__ void sumsq_kernel(const T* __restrict__ x, size_t n, float* __restric
   if (threadIdx.x == 0) atomicAdd(out, s);
 }
 
-static inline int grid_for(size_t work_items, int threads, int max_blocks = 148 * 8) {
+static inline int grid_for(size_t work_items, int threads, int max_blocks = 132 * 8) {
   size_t b = (work_items + threads - 1) / threads;
   if (b < 1) b = 1;
   return (int)(b > (size_t)max_blocks ? max_blocks : b);
@@ -737,7 +737,7 @@ using namespace b200;
 extern "C" int b200_rmsnorm_fwd(const void* x, const void* w, void* y, float* rstd, int M, int D, float eps,
                                 cudaStream_t s) {
   if (D % 8 || D > NT * 8 * MAXC) return -1;
-  const int grid = M < 148 * 6 ? M : 148 * 6;
+  const int grid = M < 132 * 6 ? M : 132 * 6;
   const int nc = (D + NT * 8 - 1) / (NT * 8);
 #define B200_RMS_FWD(NCV)                                                                                     \
   rmsnorm_fwd_kernel<NCV><<<grid, NT, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)w, (__nv_bfloat16*)y, \
@@ -746,7 +746,7 @@ extern "C" int b200_rmsnorm_fwd(const void* x, const void* w, void* y, float* rs
 #undef B200_RMS_FWD
   CK();
 }
-extern "C" int b200_rmsnorm_bwd_grid(int M) { return M < 148 * 4 ? M : 148 * 4; }
+extern "C" int b200_rmsnorm_bwd_grid(int M) { return M < 132 * 4 ? M : 132 * 4; }
 extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, const float* rstd, const void* dres,
                                 void* dx, float* dw_part, float* dw, int M, int D, cudaStream_t s) {
   if (D % 8 || D > NT * 8 * MAXC) return -1;
@@ -764,7 +764,7 @@ extern "C" int b200_rmsnorm_bwd(const void* dy, const void* x, const void* w, co
 extern "C" int b200_add_rmsnorm_fwd(const void* x, const float* res, const void* w, void* y, float* res_out, float* rstd,
                                     int M, int D, float eps, cudaStream_t s) {
   if (D % 8 || D > NT * 8 * MAXC) return -1;
-  add_rmsnorm_fwd_kernel<<<M < 148 * 8 ? M : 148 * 8, NT, 0, s>>>((const __nv_bfloat16*)x, res, (const __nv_bfloat16*)w,
+  add_rmsnorm_fwd_kernel<<<M < 132 * 8 ? M : 132 * 8, NT, 0, s>>>((const __nv_bfloat16*)x, res, (const __nv_bfloat16*)w,
                                                                  (__nv_bfloat16*)y, res_out, rstd, M, D, eps);
   CK();
 }
@@ -779,7 +779,7 @@ extern "C" int b200_rmsnorm_bwd_f32(const void* dy, const float* x, const void* 
 extern "C" int b200_rmsnorm_gated_fwd(const void* x, const void* z, const void* w, void* y, float* rstd, int M, int D,
                                       float eps, cudaStream_t s) {
   if (D % 8 || D > NT * 8 * MAXC) return -1;
-  rmsnorm_gated_fwd_kernel<<<M < 148 * 8 ? M : 148 * 8, NT, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)z,
+  rmsnorm_gated_fwd_kernel<<<M < 132 * 8 ? M : 132 * 8, NT, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)z,
                                                                    (const __nv_bfloat16*)w, (__nv_bfloat16*)y, rstd, M, D, eps);
   CK();
 }
@@ -797,7 +797,7 @@ extern "C" int b200_rope(void* qkv, const float* table, int M, int seq_len, int 
                          int rot, int inverse, int pos_offset, int interleaved, cudaStream_t s) {
   if (rot % 16 || hd % 8 || row_stride % 8) return -1;
   if (interleaved) {
-    rope_kernel<<<(M < 148 * 8 ? M : 148 * 8), 256, 0, s>>>((__nv_bfloat16*)qkv, table, M, seq_len, row_stride, nrot_heads,
+    rope_kernel<<<(M < 132 * 8 ? M : 132 * 8), 256, 0, s>>>((__nv_bfloat16*)qkv, table, M, seq_len, row_stride, nrot_heads,
                                                      hd, rot, inverse ? -1.f : 1.f, pos_offset);
   } else {
     size_t total = (size_t)M * nrot_heads * (rot / 16);
@@ -862,7 +862,7 @@ extern "C" int b200_count_valid(const long long* labels, int M, long long ignore
 extern "C" int b200_ce_grad_inplace(void* logits, const long long* labels, const float* n_valid, float* loss_sum,
                                     int rows, int V, int ld, long long ignore, cudaStream_t s) {
   if (V % 8 || ld % 8) return -1;
-  ce_grad_inplace_kernel<<<rows < 148 * 8 ? rows : 148 * 8, NT, 0, s>>>((__nv_bfloat16*)logits, labels, n_valid,
+  ce_grad_inplace_kernel<<<rows < 132 * 8 ? rows : 132 * 8, NT, 0, s>>>((__nv_bfloat16*)logits, labels, n_valid,
                                                                        loss_sum, rows, V, ld, ignore);
   CK();
 }
@@ -870,7 +870,7 @@ extern "C" int b200_adamw(float* master, const void* grad, int grad_is_bf16, flo
                           long long n, float lr, float b1, float b2, float eps, float wd, float bc1, float bc2_sqrt,
                           const float* grad_scale, cudaStream_t s) {
   if (n % 4) return -1;
-  int g = grid_for((size_t)n / 4, 256, 148 * 16);
+  int g = grid_for((size_t)n / 4, 256, 132 * 16);
   if (grad_is_bf16)
     adamw_kernel<__nv_bfloat16><<<g, 256, 0, s>>>(master, (const __nv_bfloat16*)grad, m, v, (__nv_bfloat16*)lowp,
                                                   (size_t)n, lr, b1, b2, eps, wd, bc1, bc2_sqrt, grad_scale);
@@ -881,7 +881,7 @@ extern "C" int b200_adamw(float* master, const void* grad, int grad_is_bf16, flo
 }
 extern "C" int b200_sumsq(const void* x, int is_bf16, long long n, float* out, cudaStream_t s) {
   if (reinterpret_cast<uintptr_t>(x) & 15) return -1;
-  int g = grid_for((size_t)n / 16, 256, 148 * 8);
+  int g = grid_for((size_t)n / 16, 256, 132 * 8);
   if (is_bf16) sumsq_kernel<__nv_bfloat16><<<g, 256, 0, s>>>((const __nv_bfloat16*)x, (size_t)n, out);
   else sumsq_kernel<float><<<g, 256, 0, s>>>((const float*)x, (size_t)n, out);
   CK();

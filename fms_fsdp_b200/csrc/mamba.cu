@@ -1,4 +1,4 @@
-// Mamba-path kernels (sm_100a): depthwise causal conv1d (+SiLU) forward / backward on channels-last
+// Mamba-path kernels (sm_90a): depthwise causal conv1d (+SiLU) forward / backward on channels-last
 // activations [B*S, C] (SURVEY.md M2).  The SSD / selective scans live in ssd.cu.
 #include "common.cuh"
 

@@ -2,7 +2,7 @@
 //
 //   h_t = exp(delta_t A) h_{t-1} + delta_t u_t B_t ;   y_t = C_t . h_t + D u_t ;   y_t *= silu(z_t)
 //
-// Not GEMM-shaped (d_state = 16): a bandwidth/latency kernel.  B200 mapping: CTA = 32 channels x the whole sequence of
+// Not GEMM-shaped (d_state = 16): a bandwidth/latency kernel.  H100 mapping: CTA = 32 channels x the whole sequence of
 // one batch element; WARP = one channel, LANE = one of 32 consecutive timesteps; the recurrence over a 32-step block is
 // an affine inclusive scan done with 5 shuffle rounds per state, blocks are chained through a per-warp carry.  Tiles of
 // [32 t x 32 d] go through shared memory so every global access is a coalesced 64-byte row segment, and B_t / C_t

@@ -1,7 +1,7 @@
 // Mamba2 state-space-dual (SSD) chunk scan, forward and backward (SURVEY.md M3; reference: mamba_ssm's Triton
 // ssd_chunk_state / ssd_state_passing / ssd_bmm / ssd_chunk_scan / ssd_combined).
 //
-// All GEMM-shaped work runs on the tcgen05 GEMM in batched mode (gemm_sm100.cu, BATCH=true): per 128-token chunk
+// All GEMM-shaped work runs on the wgmma GEMM in batched mode (gemm_sm90.cu, BATCH=true): per 128-token chunk
 //   CB = C_c B_c^T,  Y_diag = (CB o decay-mask_h) X_h,  S_c = B_c^T (X o dt o decay),  Y_off = C_c prev_c
 // with the per-head products folded into the N (or K) dimension wherever the other operand is shared by the heads.
 // This file holds the glue between those GEMMs: dt softplus + in-chunk cumsum, the per-head decay mask, the
@@ -338,7 +338,7 @@ __global__ void ssd_dt_bwd_kernel(const __nv_bfloat16* __restrict__ dt, const fl
 
 static inline int ew_grid(size_t work, int threads) {
   size_t b = (work + threads - 1) / threads;
-  return (int)(b > 148 * 16 ? 148 * 16 : (b < 1 ? 1 : b));
+  return (int)(b > 132 * 16 ? 132 * 16 : (b < 1 ? 1 : b));
 }
 
 }  // namespace b200

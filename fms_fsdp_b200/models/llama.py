@@ -1,4 +1,4 @@
-"""LLaMA for the B200 engine.
+"""LLaMA for the engine.
 
 State-dict names, fused-weight layout, initialisation and numerics contract follow the
 ibm-fms LLaMA that the reference trains (SURVEY.md §2.4 E2; names evidenced by reference
@@ -7,7 +7,7 @@ attn.dense, ff_ln, ff_sub_layer.wg1_fused, ff_sub_layer.w2}``, ``dec_norm``; RoP
 interleaved-pair convention; RMSNorm in fp32; SwiGLU on ``[gate | up]``.
 
 The architecture is *not* a module-per-op graph: each block is one straight-line sequence of
-engine ops (``fms_fsdp_b200.ops``) that run as sm_100a kernels on GPU, and the model exposes
+engine ops (``fms_fsdp_b200.ops``) that run as sm_90a kernels on GPU, and the model exposes
 ``engine_units()`` so the sharded runtime can schedule gather / compute / reduce per unit.
 """
 from __future__ import annotations

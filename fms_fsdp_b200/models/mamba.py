@@ -1,4 +1,4 @@
-"""Mamba2-hybrid language model for the B200 engine.
+"""Mamba2-hybrid language model for the engine.
 
 Stands in for what the reference imports from ``mamba_ssm`` (``MambaConfig``, ``MambaLMHeadModel``,
 ``Block``, ``Mamba2``, ``MHA``, ``GatedMLP`` -- reference ``main_training_mamba.py:8-10,55,65-67``;
@@ -6,10 +6,10 @@ SURVEY.md §2.4 E3, §2.5(b)).  State-dict names follow mamba_ssm (``backbone.em
 ``backbone.layers.N.{norm,mixer,norm2,mlp}``, ``backbone.norm_f``, ``lm_head``) so
 ``fms_to_hf_mamba`` emits the familiar ``config.json`` + ``pytorch_model.bin``.
 
-Every block is a straight line of engine ops (``fms_fsdp_b200.ops``): tcgen05 GEMMs for
+Every block is a straight line of engine ops (``fms_fsdp_b200.ops``): wgmma GEMMs for
 in/out projections and the gated MLP, fused causal-conv1d+SiLU, the SSD chunked scan, gated
 RMSNorm, the fp32 residual stream with fused add+norm, and -- for the attention layers of the
-hybrid -- the same tcgen05 flash attention as Llama with partial (half-split) rotary.
+hybrid -- the same wgmma flash attention as Llama with partial (half-split) rotary.
 """
 from __future__ import annotations
 

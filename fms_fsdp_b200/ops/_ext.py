@@ -1,4 +1,4 @@
-"""Loader for the in-tree sm_100a extension (``fms_fsdp_b200/_C*.so``).
+"""Loader for the in-tree sm_90a extension (``fms_fsdp_b200/_C*.so``).
 
 The extension is built by ``__graft_entry__.build()`` / ``python -m fms_fsdp_b200.build``.
 On a machine with a GPU the ops in this package *require* it: there is no silent
@@ -37,7 +37,7 @@ def require():
     m = load()
     if m is None:
         raise RuntimeError(
-            "fms_fsdp_b200._C (sm_100a kernels) is not built/loadable: "
+            "fms_fsdp_b200._C (sm_90a kernels) is not built/loadable: "
             f"{_err!r}. Run `python -c 'import __graft_entry__ as g; g.build()'`."
         )
     return m

@@ -1,6 +1,6 @@
-"""sm_100a primitive set (same signatures as ``torch_kernels``), backed by ``fms_fsdp_b200._C``.
+"""sm_90a primitive set (same signatures as ``torch_kernels``), backed by ``fms_fsdp_b200._C``.
 
-Every function here launches hand-written kernels from ``csrc/`` (tcgen05 GEMM / flash attention,
+Every function here launches hand-written kernels from ``csrc/`` (wgmma GEMM / flash attention,
 fused elementwise, peer-memory collectives).  ``launch_count()`` reports how many of OUR kernels
 were launched (bench.py's ``gpu_launches``).
 """
@@ -16,14 +16,10 @@ NAME = "cuda"
 _C = _ext.require()
 
 _LAYOUT = {"nt": 0, "nn": 1, "tn": 2}
-# attention implementation: "tcgen05" (ours) | "sdpa" (library fallback, debugging only)
-ATTN_IMPL = os.environ.get("FMS_B200_ATTN_IMPL", "tcgen05")
-GEMM_IMPL = os.environ.get("FMS_B200_GEMM_IMPL", "tcgen05")  # "cublas" = library fallback, debugging only
-# pairs (of every 4) of softmax exponentials computed on the FMA pipe (packed FFMA2 polynomial) instead of the MUFU
-# (measured, profiles/attn_bench_r2.json: the split is performance-neutral -- the row owners are bound by the dependency
-# chain S -> exp -> P -> next MMA, not by MUFU throughput -- so the defaults stay at 0 / 1)
-_C.set_attn_poly(int(os.environ.get("FMS_B200_ATTN_POLY_FWD", "0")), int(os.environ.get("FMS_B200_ATTN_POLY_BWD", "1")))
-_C.set_gemm_2cta(os.environ.get("FMS_B200_GEMM_2CTA", "1") == "1")  # CTA-pair (cta_group::2) GEMM for M >= 256
+# attention implementation: "wgmma" (ours) | "sdpa" (library fallback, debugging only)
+ATTN_IMPL = os.environ.get("FMS_B200_ATTN_IMPL", "wgmma")
+GEMM_IMPL = os.environ.get("FMS_B200_GEMM_IMPL", "wgmma")  # "cublas" = library fallback, debugging only
+_C.set_gemm_2cta(os.environ.get("FMS_B200_GEMM_2CTA", "1") == "1")  # fused-epilogue GEMM paths (RoPE, SwiGLU, push, fp8) for M >= 256
 
 
 def launch_count() -> int:
@@ -137,7 +133,7 @@ def _try_fused_gather(a, b, layout, out, epi, residual) -> bool:
 
 class PushTarget:
     """"Output" of a wgrad GEMM whose epilogue writes every tile into the staging slots of the rank that owns that
-    slice of the unit's flat gradient (fused GEMM -> reduce-scatter, SURVEY.md N8; ``csrc/gemm2_sm100.cu`` P_EPI_PUSH).
+    slice of the unit's flat gradient (fused GEMM -> reduce-scatter, SURVEY.md N8; ``csrc/gemm_sm90.cu`` EPI_PUSH).
     ``table``: int64 device tensor of the ranks' staging-buffer addresses; ``n``: elements per shard; ``off``: element
     offset of this weight inside the flat unit."""
     __slots__ = ("table", "n", "off", "rank", "shape", "dtype", "world")
@@ -161,7 +157,7 @@ PUSH_STATS = {"gemms": 0, "with_gather": 0}
 
 
 def push_eligible_shape(shape) -> bool:
-    """Weight shapes the push epilogue handles (CTA-pair wgrad GEMM, 16-byte vectors never straddle an owner)."""
+    """Weight shapes the push epilogue handles (wgrad GEMM, 8-element vectors never straddle an owner)."""
     return len(shape) == 2 and shape[0] >= 256 and shape[0] % 8 == 0 and shape[1] % 8 == 0
 
 
@@ -191,7 +187,7 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
         return _gemm_push(a, b, out)
     if rope is not None:
         M0 = a.shape[0]
-        ok = (GEMM_IMPL == "tcgen05" and layout == "nt" and a.dtype == b.dtype == torch.bfloat16 and residual is None
+        ok = (GEMM_IMPL == "wgmma" and layout == "nt" and a.dtype == b.dtype == torch.bfloat16 and residual is None
               and not accumulate and M0 >= 256 and M0 % 8 == 0 and _C.get_gemm_2cta() and rope[2] % 8 == 0
               and a.shape[1] % 8 == 0 and b.shape[0] % 8 == 0 and out_dtype in (None, torch.bfloat16)
               and (out is None or out.dtype == torch.bfloat16))
@@ -199,7 +195,7 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
             y = gemm(a, b, layout, out=out, accumulate=accumulate, residual=residual, out_dtype=out_dtype)
             table, S, hd, H, KVH = rope
             return rope_(y, table, S, H, KVH, hd)
-    if GEMM_IMPL != "tcgen05" or a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
+    if GEMM_IMPL != "wgmma" or a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16:
         return _fallback("gemm").gemm(a, b, layout, out=out, accumulate=accumulate, residual=residual, out_dtype=out_dtype)
     if layout == "nt":
         M, N = a.shape[0], b.shape[0]
@@ -234,22 +230,19 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
 
 # -------------------------------------------------------- gate/up GEMM + SwiGLU, down-proj dgrad + SwiGLU backward
 FUSE_SWIGLU = os.environ.get("FMS_B200_FUSE_SWIGLU", "1") == "1"
-# Measured on Llama2-7B, 1 GPU, same box (profiles/step_kernel_table_1gpu_swiglu_{fused,unfused}_r2.txt, ab_1gpu_swiglu_*):
-# forward fusion +97 us in the gate/up GEMM, -112 us activation kernel.  The first backward epilogue read gate/up in
-# 32-column steps (every 128-byte line fetched twice, loads issued after the TMEM wait): 904 us vs 560 + 155 us unfused;
-# with 64-column steps and the loads issued before the TMEM wait the step time equals the unfused one (329.7 vs 329.4 ms)
-# while dS [M, F] never reaches memory -- on by default.
+# The SwiGLU activation and its gradient run in the epilogues of the gate/up and down-projection GEMMs, so the
+# activation and dS [M, F] never make a round trip through memory -- on by default.
 FUSE_SWIGLU_BWD = os.environ.get("FMS_B200_FUSE_SWIGLU_BWD", "1") == "1"
 
 
 def _swiglu_fusable(x, F):
-    return (FUSE_SWIGLU and GEMM_IMPL == "tcgen05" and x.dtype == torch.bfloat16 and x.shape[0] >= 256 and x.shape[0] % 8 == 0
+    return (FUSE_SWIGLU and GEMM_IMPL == "wgmma" and x.dtype == torch.bfloat16 and x.shape[0] >= 256 and x.shape[0] % 8 == 0
             and _C.get_gemm_2cta())
 
 
 def gated_up_fwd(x, w, gate_first=True):
-    """(gu [M, 2F] bf16, silu(gate) * up [M, F]): the activation is the EPILOGUE of the gate/up GEMM -- a CTA pair's
-    accumulator holds gate and up of the same 128 features side by side (csrc/gemm2_sm100.cu P_EPI_SWIGLU)."""
+    """(gu [M, 2F] bf16, silu(gate) * up [M, F]): the activation is the EPILOGUE of the gate/up GEMM -- a tile's
+    accumulator holds gate and up of the same 64 features side by side (csrc/gemm_sm90.cu EPI_SWIGLU)."""
     F = w.shape[0] // 2
     if not (_swiglu_fusable(x, F) and w.dtype == torch.bfloat16 and F % 128 == 0 and x.shape[1] % 8 == 0):
         gu = gemm(x, w, "nt")
@@ -267,7 +260,7 @@ def gated_up_fwd(x, w, gate_first=True):
 
 def gated_down_bwd(dy, w2, gu, gate_first=True):
     """d(gu) [M, 2F] = swiglu_bwd(dy @ w2, gu) with the SwiGLU backward as the epilogue of the dgrad GEMM: dS = dy @ w2
-    never reaches memory (csrc/gemm2_sm100.cu P_EPI_SWIGLU_BWD)."""
+    never reaches memory (csrc/gemm_sm90.cu EPI_SWIGLU_BWD)."""
     F = w2.shape[1]
     if not (FUSE_SWIGLU_BWD and _swiglu_fusable(dy, F) and w2.dtype == gu.dtype == torch.bfloat16 and F % 8 == 0 and dy.shape[1] % 8 == 0
             and gu.is_contiguous()):
@@ -291,7 +284,7 @@ def quant_rowwise_e4m3(x):
 
 
 def gemm_fp8(aq, bq, sa, sb, out=None):
-    """e4m3 x e4m3 -> bf16 on the tensor cores (tcgen05.mma kind::f8f6f4, CTA pair), row / column scales in the epilogue."""
+    """e4m3 x e4m3 -> bf16 on the tensor cores (wgmma e4m3), row / column scales in the epilogue."""
     M, K = aq.shape
     N = bq.shape[0]
     if out is None:
@@ -369,7 +362,7 @@ def _sdpa_fwd(qkv, B, S, H, KVH, hd, scale):
 
 
 def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
-    if ATTN_IMPL == "tcgen05" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
+    if ATTN_IMPL == "wgmma" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
         o, lse = _C.attn_fwd(qkv.contiguous(), B, S, H, KVH, hd, float(scale))
         return o, lse
     if ATTN_IMPL == "sdpa":
@@ -380,7 +373,7 @@ def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
 def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=None):
     """``rope_table``: the forward applied RoPE (full head_dim, interleaved) to q, k before this attention; return the
     gradient of the UN-rotated projection (inverse rotation fused into the dq / dk epilogues)."""
-    if ATTN_IMPL == "tcgen05" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
+    if ATTN_IMPL == "wgmma" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
         return _C.attn_bwd(do.contiguous(), qkv.contiguous(), o, lse, B, S, H, KVH, hd, float(scale), rope_table)
     if rope_table is not None:
         g = attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal)
@@ -512,7 +505,7 @@ def _f32c(t):
 
 
 def ssd_scan_fwd(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus=True):
-    """Mamba2 SSD scan (csrc/ssd.cu + batched tcgen05 GEMMs); 128-token internal chunks whatever ``chunk_size``."""
+    """Mamba2 SSD scan (csrc/ssd.cu + batched wgmma GEMMs); 128-token internal chunks whatever ``chunk_size``."""
     if not _ssd_native_ok(x, dt, Bm, Cm, seq_len):
         return _fallback("ssd_scan_chunked").ssd_scan_chunked(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus)
     return _C.ssd_scan_fwd(x.contiguous(), dt.contiguous(), _f32c(A), Bm.contiguous(), Cm.contiguous(), _f32c(D),

@@ -1,7 +1,7 @@
 """Differentiable ops of the engine.
 
 Every op is a ``torch.autograd.Function`` with a hand-written backward that calls the *same
-primitive set* on both back-ends: ``cuda_kernels`` (sm_100a, tcgen05/TMA) for CUDA tensors and
+primitive set* on both back-ends: ``cuda_kernels`` (sm_90a, wgmma/TMA) for CUDA tensors and
 ``torch_kernels`` (ATen oracle) for CPU tensors.  Weights are read through the live
 ``Parameter.data`` in backward (never through autograd-saved views) because the sharded runtime
 re-points parameters at a freshly gathered buffer between forward and backward; weight
@@ -32,7 +32,7 @@ def get_kernel_path() -> str:
 
 
 def kernels_for(t: torch.Tensor):
-    """Primitive namespace for tensor ``t``: CUDA tensors *require* the sm_100a extension."""
+    """Primitive namespace for tensor ``t``: CUDA tensors *require* the sm_90a extension."""
     if t.is_cuda and _KERNEL_PATH != "torch":
         if not _ext.available():
             if _ext.allow_torch_fallback():

@@ -1,6 +1,6 @@
 """ATen implementations of every engine primitive (forward *and* hand-derived backward).
 
-Two jobs: (1) the CPU/gloo plumbing path and numerical oracle for the sm_100a kernels
+Two jobs: (1) the CPU/gloo plumbing path and numerical oracle for the sm_90a kernels
 (tests compare ``cuda_kernels.X`` against ``torch_kernels.X`` and both against autograd of
 the naive formula); (2) executable documentation of exactly what each CUDA kernel computes.
 Signatures are identical to ``cuda_kernels``.
@@ -230,7 +230,7 @@ def quant_rowwise_e4m3(x):
 
 
 def gemm_fp8(aq, bq, sa, sb, out=None):
-    """C = (A_q B_q^T) * sa[:, None] * sb[None, :] in bf16 (oracle of csrc/gemm2_sm100.cu b200_gemm2_fp8)."""
+    """C = (A_q B_q^T) * sa[:, None] * sb[None, :] in bf16 (oracle of csrc/gemm_sm90.cu b200_gemm2_fp8)."""
     a = aq.view(torch.float8_e4m3fn).float()
     b = bq.view(torch.float8_e4m3fn).float()
     y = ((a @ b.t()) * sa[:, None] * sb[None, :]).to(torch.bfloat16)

@@ -209,7 +209,7 @@ class ShardedModel(nn.Module):
         self._grad_pool: Dict[Tuple, List[_Buf]] = {}
         self._pool_made: Dict[Tuple, int] = {}
         self._bwd_gather_split = float(os.environ.get("FMS_B200_AG_SPLIT_BWD", "1.0"))
-        # backward knobs (measured in profiles/README.md): gradient-buffer pool depth (1 = the block's backward waits for
+        # backward knobs: gradient-buffer pool depth (1 = the block's backward waits for
         # the previous unit's reduce, 2 = they overlap) and whether backward re-gathers ride inside the GEMMs
         self._grad_pool_depth = int(os.environ.get("FMS_B200_GRAD_POOL", "1"))
         self.poison_released_params = os.environ.get("FMS_B200_POISON", "0") == "1"
@@ -477,7 +477,7 @@ class ShardedModel(nn.Module):
         u.bind_grads(u.full_grad.t)
 
     def _push_eligible(self, u: ShardUnit) -> bool:
-        """Block units whose every parameter is a norm-style vector or a weight matrix large enough for the CTA-pair
+        """Block units whose every parameter is a norm-style vector or a weight matrix large enough for the fused-epilogue
         wgrad GEMM (LLaMA blocks); the root unit (embedding / tied or chunk-accumulated head) and units with other
         parameter kinds (Mamba conv / SSM tensors) keep the pull path."""
         if u is self.root:

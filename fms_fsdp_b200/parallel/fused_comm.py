@@ -1,5 +1,5 @@
 """NVLink / NVSwitch collectives of the sharded runtime: our own peer-memory kernels, no NCCL on the
-parameter / gradient paths (SURVEY.md §5.8 "B200-native design").
+parameter / gradient paths (SURVEY.md §5.8).
 
 * buffers that peers must reach (compute-dtype parameter shards, unsharded gradient buffers, HSDP gradient
   shards) are allocated from torch symmetric memory and rendezvoused once; we keep, per buffer, a device
@@ -7,7 +7,7 @@ parameter / gradient paths (SURVEY.md §5.8 "B200-native design").
 * ``all_gather``      = pull kernel (``csrc/comm.cu::p2p_allgather_kernel``): every rank copies the 7 remote
   shards with 16-byte peer loads, rotated start so all inbound NVLink flows are busy;
 * gradients of LLaMA-style blocks never exist unsharded: the wgrad GEMM epilogue PUSHES each tile into the owning
-  rank's staging slot ``[src rank][shard]`` (``csrc/gemm2_sm100.cu`` ``P_EPI_PUSH``); after ONE cross-rank flag round
+  rank's staging slot ``[src rank][shard]`` (``csrc/gemm_sm90.cu`` ``EPI_PUSH``); after ONE cross-rank flag round
   per unit the owner sums its ``world`` local slots in fp32, scales by 1/world, writes the fp32 shard and accumulates
   ||g||^2 in the same pass (``reduce_pushed``; K11 folded into N8) -- no NVLink traffic outside the GEMMs;
 * ``reduce_scatter``  = one-shot pull-reduce for everything else (root unit, Mamba blocks): rank r sums slice r of all
@@ -123,8 +123,9 @@ class FusedCollectives:
         self._anchor = torch.zeros(1, device=device)
         self._slice_tables: Dict[Tuple[int, int], torch.Tensor] = {}
         self._ag_state: Dict[int, list] = {}
-        # CTA cap of the reduce kernels (csrc/comm.cu); throttling them was measured slower (2 GPUs: 354 -> 361 ms/step)
-        self.C.set_reduce_ctas(int(os.environ.get("FMS_B200_REDUCE_CTAS", "296")))
+        # CTA cap of the reduce kernels (csrc/comm.cu): by default two CTAs per SM of this GPU
+        sms = torch.cuda.get_device_properties(device).multi_processor_count
+        self.C.set_reduce_ctas(int(os.environ.get("FMS_B200_REDUCE_CTAS", str(2 * sms))))
         self._own_scalar = os.environ.get("FMS_B200_OWN_SCALAR_ALLREDUCE", "1") == "1"
         # CTA cap of the local slot sum (runs under the backward GEMMs; 0 = same as the pull kernels)
         self._slotsum_ctas = int(os.environ.get("FMS_B200_SLOTSUM_CTAS", "0"))

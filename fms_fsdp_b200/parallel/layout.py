@@ -3,7 +3,7 @@
 A *unit* (one transformer/Mamba block, or the root = embedding + head + final norm; reference
 wrapping policy ``fms_fsdp/policies/wrapping.py:6-14``) owns one flat buffer.  Each parameter
 starts at a 128-byte-aligned element offset (TMA global addresses need 16 B; 128 B keeps every
-weight tile sector-aligned for the tcgen05 GEMMs), the total is right-padded to a multiple of
+weight tile sector-aligned for the TMA-fed GEMMs), the total is right-padded to a multiple of
 ``shard_world * align`` and cut into ``shard_world`` equal contiguous 1-D chunks (the torch
 FSDP1 FlatParameter convention, SURVEY.md §2.4 E1) so reduce-scatter / all-gather are single
 contiguous transfers per peer.

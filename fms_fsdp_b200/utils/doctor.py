@@ -1,6 +1,6 @@
 """Environment check before a run:  ``python -m fms_fsdp_b200.utils.doctor``
 
-Reports, without starting a job: Python / torch / CUDA versions, whether the in-tree sm_100a extension is built and loads, the
+Reports, without starting a job: Python / torch / CUDA versions, whether the in-tree sm_90a extension is built and loads, the
 visible GPUs (name, compute capability, memory, SM count), peer access between every pair of GPUs (the NVLink collectives need
 it), NCCL and symmetric-memory availability, the measured roofline file the MFU line uses, and the reference install the bench's
 reference arm needs.  Exit status 1 if something that a GPU training run requires is missing; on a machine without a GPU it
@@ -56,9 +56,9 @@ def collect() -> dict:
     if not info["extension_built"] or not info["extension_loads"]:
         info["problems"].append("fms_fsdp_b200/_C.so missing or not loadable: run python -c 'import __graft_entry__ as g; g.build()'")
     for g in info["gpus"]:
-        if g["capability"] != "10.0":
+        if g["capability"] != "9.0":
             info["problems"].append(f"GPU {g['index']} ({g['name']}) is sm_{g['capability'].replace('.', '')}; the kernels are "
-                                    "compiled for sm_100a only")
+                                    "compiled for sm_90a only")
     no_peer = [(a, b) for a in range(n) for b in range(n) if a != b and not torch.cuda.can_device_access_peer(a, b)]
     info["peer_access_all_pairs"] = not no_peer
     if no_peer:

@@ -1,4 +1,4 @@
-"""Per-GPU memory plan of a Llama run on this engine -- "does this configuration fit in 180 GB of HBM3e, and what should be
+"""Per-GPU memory plan of a Llama run on this engine -- "does this configuration fit in the 80 GB of HBM3 of an H100, and what should be
 recomputed?" answered before a job is queued.
 
     python -m fms_fsdp_b200.utils.memory_plan --model_variant=llama2_13b --gpus=8 --sharding_strategy=fsdp \
@@ -16,9 +16,10 @@ The numbers follow what the runtime allocates (``parallel/engine.py``) and what 
   statistics; a recomputed block keeps its input only, one block's worth of activations is live while it is recomputed;
 * head: the final hidden states, their gradient and one [4096, V] logits chunk (+ its gradient in place).
 
-Checked against the measured peak of the caching allocator: Llama2-7B, 1 GPU, no recomputation = 133.53 GiB
-(``profiles/bench1_on8box_r2.log``), plan 133.0 GiB (``tests/test_config.py``).  Symmetric-memory buffers of the peer
-collectives are not visible to the caching allocator; ``bench.py`` therefore also reports ``mem_device_gb``.
+Checked against the measured peak of the caching allocator: Llama2-1.4B, 1 H100 80GB HBM3 (400 W limit), seq 4096,
+batch 2, no recomputation = 31.19 GiB (``bench.py --gpus 1``), plan 31.18 GiB (``tests/test_config.py``).
+Symmetric-memory buffers of the peer collectives are not visible to the caching allocator; ``bench.py`` therefore also
+reports ``mem_device_gb``.
 """
 from __future__ import annotations
 
@@ -26,7 +27,7 @@ from dataclasses import dataclass, field
 from typing import Dict
 
 GiB = float(2 ** 30)
-HBM_GIB_B200 = 180e9 / GiB      # 180 GB of HBM3e (the driver, context and NCCL take a few GiB of it)
+HBM_GIB = 80e9 / GiB           # 80 GB of HBM3 on an H100 (the driver, context and NCCL take a few GiB of it)
 
 
 @dataclass
@@ -40,7 +41,7 @@ class MemoryPlan:
     def total_gib(self) -> float:
         return sum(self.parts_gib.values())
 
-    def fits(self, budget_gib: float = HBM_GIB_B200, headroom: float = 0.92) -> bool:
+    def fits(self, budget_gib: float = HBM_GIB, headroom: float = 0.92) -> bool:
         """``headroom``: fraction of the device the plan may take (allocator fragmentation, CUDA context, NCCL buffers)."""
         return self.total_gib <= budget_gib * headroom
 
@@ -48,7 +49,7 @@ class MemoryPlan:
         w = max(len(k) for k in self.parts_gib)
         rows = [f"{k:<{w}}  {v:8.2f} GiB" for k, v in self.parts_gib.items()]
         rows.append(f"{'total':<{w}}  {self.total_gib:8.2f} GiB   ({'fits' if self.fits() else 'DOES NOT FIT'} in "
-                    f"{HBM_GIB_B200:.0f} GiB at 92 % usable)")
+                    f"{HBM_GIB:.0f} GiB at 92 % usable)")
         return "\n".join(rows)
 
 

@@ -58,7 +58,7 @@ def torchrun_env():
 
 # ----------------------------------------------------------------------------------------- policies
 def get_mixed_precision_policy(cfg, rank):
-    """bf16 everywhere when the device supports it (always on B200), fp16 otherwise, None when off.
+    """bf16 everywhere when the device supports it (always on H100), fp16 otherwise, None when off.
     Reference: ``fms_fsdp/utils/train_utils.py:192-214``."""
     if not cfg.mixed_precision:
         return None
@@ -142,7 +142,7 @@ def peak_tflops() -> float:
                 return float(json.load(f)["bf16_tflops_sustained"])
         except Exception:
             continue
-    return 1400.0
+    return 989.0   # H100 SXM data-sheet dense bf16 (700 W); power-limited cards reach less
 
 
 # ------------------------------------------------------------------------------------------ trackers

@@ -6,7 +6,7 @@
 Every ``train_config`` field is a ``--field=value`` flag.  Same flow as the reference -- config, seeds,
 process group, policies, model (optionally on the meta device), data loader, sharded wrap, RoPE table
 precompute, selective recomputation, AdamW(0.9, 0.95, wd 0.1), checkpoint auto-resume, LR schedule,
-profiler, train -- on the B200-native engine instead of torch FSDP + torch.compile.
+profiler, train -- on the H100-native engine instead of torch FSDP + torch.compile.
 """
 import os
 
@@ -99,7 +99,7 @@ def main(**kwargs):
         print(f"--> sharded runtime: {model.extra_repr()}")
         if cfg.use_torch_compile:
             print("--> use_torch_compile is accepted for compatibility; this engine runs hand-written fused "
-                  "sm_100a kernels and has no tracing compiler")
+                  "sm_90a kernels and has no tracing compiler")
 
     optimizer = ShardedAdamW(model, lr=cfg.learning_rate, betas=(0.9, 0.95), weight_decay=0.1)
 

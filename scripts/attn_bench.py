@@ -1,6 +1,6 @@
-"""Attention kernels at the headline shape (B2 H32 S4096 hd128, causal): ours (per FMA-pipe exponential split) vs the
-library (cuDNN / flash SDPA through torch), forward and backward, plus numerics vs the fp32 oracle at a small shape.
-Writes gpurun_out/attn_bench.json.   usage: python scripts/attn_bench.py [fwd_pairs,...] [bwd_pairs,...]"""
+"""Attention kernels at the headline shape (B2 H32 S4096 hd128, causal): ours vs the library (cuDNN / flash SDPA through
+torch), forward and backward, plus numerics vs the fp32 oracle at a small shape.
+Writes $DIAG_OUT/attn_bench.json (default diag_out/ in the repository root).   usage: python scripts/attn_bench.py"""
 import json
 import os
 import sys
@@ -34,8 +34,6 @@ def rel(a, b):
     return ((a - b).abs().max() / b.abs().max().clamp(min=1e-6)).item()
 
 
-fwd_list = [int(x) for x in (sys.argv[1] if len(sys.argv) > 1 else "0,2,3").split(",")]
-bwd_list = [int(x) for x in (sys.argv[2] if len(sys.argv) > 2 else "0,2,3").split(",")]
 torch.manual_seed(0)
 # numerics (small, multi-tile, GQA)
 B, S, H, KVH, hd = 2, 512, 4, 2, 128
@@ -43,26 +41,20 @@ qkv_s = (torch.randn(B * S, (H + 2 * KVH) * hd, device=dev) * 0.8).bfloat16()
 do_s = torch.randn(B * S, H * hd, device=dev).bfloat16()
 o0, l0 = TK.attn_fwd(qkv_s.float(), B, S, H, KVH, hd, hd ** -0.5)
 g0 = TK.attn_bwd(do_s.float(), qkv_s.float(), o0, l0, B, S, H, KVH, hd, hd ** -0.5)
-for pp in sorted(set(fwd_list + bwd_list)):
-    CK._C.set_attn_poly(pp, pp)
-    o1, l1 = CK.attn_fwd(qkv_s, B, S, H, KVH, hd, hd ** -0.5)
-    g1 = CK.attn_bwd(do_s, qkv_s, o1, l1, B, S, H, KVH, hd, hd ** -0.5)
-    out.append(dict(kind="numerics", poly_pairs=pp, o=rel(o1, o0), lse=rel(l1, l0), dqkv=rel(g1, g0)))
+o1, l1 = CK.attn_fwd(qkv_s, B, S, H, KVH, hd, hd ** -0.5)
+g1 = CK.attn_bwd(do_s, qkv_s, o1, l1, B, S, H, KVH, hd, hd ** -0.5)
+out.append(dict(kind="numerics", o=rel(o1, o0), lse=rel(l1, l0), dqkv=rel(g1, g0)))
 
 # timing at the headline shape
 B, S, H, KVH, hd = 2, 4096, 32, 32, 128
 qkv = (torch.randn(B * S, (H + 2 * KVH) * hd, device=dev) * 0.8).bfloat16()
 do = torch.randn(B * S, H * hd, device=dev).bfloat16()
 fl = 4 * B * H * S * S * hd / 2
-for pp in fwd_list:
-    CK._C.set_attn_poly(pp, -1)
-    ms = time_ms(lambda: CK.attn_fwd(qkv, B, S, H, KVH, hd, hd ** -0.5))
-    out.append(dict(kind="fwd", poly_pairs=pp, ms=ms, tflops=fl / ms / 1e9))
+ms = time_ms(lambda: CK.attn_fwd(qkv, B, S, H, KVH, hd, hd ** -0.5))
+out.append(dict(kind="fwd", ms=ms, tflops=fl / ms / 1e9))
 o1, l1 = CK.attn_fwd(qkv, B, S, H, KVH, hd, hd ** -0.5)
-for pp in bwd_list:
-    CK._C.set_attn_poly(-1, pp)
-    ms = time_ms(lambda: CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, hd ** -0.5))
-    out.append(dict(kind="bwd", poly_pairs=pp, ms=ms, tflops=2.5 * fl / ms / 1e9))
+ms = time_ms(lambda: CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, hd ** -0.5))
+out.append(dict(kind="bwd", ms=ms, tflops=2.5 * fl / ms / 1e9))
 
 # the library bar: torch SDPA per backend, forward and backward
 from torch.nn.attention import SDPBackend, sdpa_kernel
@@ -79,8 +71,9 @@ for name, be in (("cudnn", SDPBackend.CUDNN_ATTENTION), ("flash", SDPBackend.FLA
                         bwd_tflops=2.5 * fl / ms_b / 1e9))
     except Exception as ex:
         out.append(dict(kind="library", backend=name, error=repr(ex)[:300]))
-os.makedirs("gpurun_out", exist_ok=True)
-with open("gpurun_out/attn_bench.json", "w") as fh:
+out_dir = os.environ.get("DIAG_OUT") or os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "diag_out")
+os.makedirs(out_dir, exist_ok=True)
+with open(os.path.join(out_dir, "attn_bench.json"), "w") as fh:
     json.dump(out, fh, indent=1)
 for r in out:
     print(json.dumps(r))

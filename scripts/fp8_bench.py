@@ -1,4 +1,4 @@
-"""Opt-in fp8 forward path: e4m3 CTA-pair GEMM (kind::f8f6f4) and the row-wise quantisation kernel at the Llama2-7B
+"""Opt-in fp8 forward path: e4m3 wgmma GEMM and the row-wise quantisation kernel at the Llama2-7B
 forward shapes, against the bf16 GEMM of the same shape.  Writes gpurun_out/fp8_bench.json."""
 import json, os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

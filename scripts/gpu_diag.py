@@ -1,5 +1,6 @@
-"""On-box diagnostic: numerics + timing of every sm_100a kernel against the ATen oracle.
-Writes gpurun_out/diag.json (one record per check) so a single gpurun call answers many questions.
+"""GPU diagnostic: numerics + timing of every sm_90a kernel against the ATen oracle.
+Writes $DIAG_OUT/diag.json (default diag_out/ in the repository root; one record per check), so one run answers many
+questions.   usage: python scripts/gpu_diag.py [gemm] [gemm2] [elem] [attn] [ssd] [selscan] ...
 Each check is isolated in try/except; a CUDA error aborts the remaining checks of that group only
 when the context is poisoned.
 """
@@ -12,7 +13,7 @@ import traceback
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
-OUT = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "gpurun_out")
+OUT = os.environ.get("DIAG_OUT") or os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "diag_out")
 os.makedirs(OUT, exist_ok=True)
 records = []
 
@@ -57,19 +58,8 @@ def main(groups):
     torch.manual_seed(0)
     rec("env", device=torch.cuda.get_device_name(0), torch=torch.__version__)
 
-    if "probe" in groups:
-        try:
-            a = torch.randn(128, 64, device=dev).bfloat16(); b = torch.randn(64, 64, device=dev).bfloat16()
-            d = CK._C.ts_mma_probe(a, b)
-            torch.cuda.synchronize()
-            ref = a.float() @ b.float().t()
-            a_sw = a.view(128, 32, 2).flip(-1).reshape(128, 64)
-            rec("ts_mma_probe", err_low_even=relerr(d, ref), err_low_odd=relerr(d, a_sw.float() @ b.float().t()))
-        except Exception as ex:
-            rec("ts_mma_probe", ok=False, error=repr(ex)[:400])
-
     if "gemm2" in groups:
-        # CTA-pair kernel vs single-CTA kernel vs cuBLAS on training shapes
+        # the fused-epilogue GEMM entry vs cuBLAS on training shapes
         for layout, (M, N, K) in [("nt", (8192, 12288, 4096)), ("nt", (8192, 22016, 4096)), ("nt", (8192, 4096, 11008)),
                                   ("nn", (8192, 4096, 12288)), ("nn", (8192, 4096, 22016)), ("tn", (12288, 4096, 8192)),
                                   ("tn", (22016, 4096, 8192)), ("nt", (256, 512, 128)), ("nn", (512, 768, 192)), ("tn", (1000, 520, 72))]:
@@ -82,18 +72,14 @@ def main(groups):
                     a = torch.randn(K, M, device=dev).bfloat16(); b = torch.randn(K, N, device=dev).bfloat16()
                 ref = TK.gemm(a, b, layout).float()
                 r = dict(layout=layout, M=M, N=N, K=K)
-                for two in (True, False):
-                    CK._C.set_gemm_2cta(two)
-                    out = CK.gemm(a, b, layout)
-                    torch.cuda.synchronize()
-                    r["relerr_2cta" if two else "relerr_1cta"] = relerr(out, ref)
-                    if M >= 4096:
-                        ms = time_ms(lambda: CK.gemm(a, b, layout))
-                        r["tflops_2cta" if two else "tflops_1cta"] = 2 * M * N * K / ms / 1e9
+                out = CK.gemm(a, b, layout)
+                torch.cuda.synchronize()
+                r["relerr"] = relerr(out, ref)
                 if M >= 4096:
+                    ms = time_ms(lambda: CK.gemm(a, b, layout))
+                    r["tflops"] = 2 * M * N * K / ms / 1e9
                     ms = time_ms(lambda: TK.gemm(a, b, layout))
                     r["tflops_cublas"] = 2 * M * N * K / ms / 1e9
-                CK._C.set_gemm_2cta(True)
                 rec("gemm2", **r)
             except Exception as ex:
                 rec("gemm2", layout=layout, M=M, N=N, K=K, ok=False, error=repr(ex)[:400])
@@ -326,35 +312,32 @@ def main(groups):
             rec("selscan", ok=False, error=repr(ex)[:500], tb=traceback.format_exc()[-900:])
 
     if "attn" in groups:
-        for ver in ([int(x) for x in os.environ.get("DIAG_ATTN_VERS", "2").split(",")]):
-          bver = int(os.environ.get("DIAG_ATTN_BWD", "3" if ver == 2 else str(ver)))
-          CK._C.set_attn_fwd_version(ver); CK._C.set_attn_bwd_version(bver)
-          for (B, S, H, KVH, hd) in [(1, 128, 1, 1, 128), (2, 256, 4, 2, 128), (1, 384, 2, 1, 128), (1, 512, 2, 2, 64), (2, 4096, 32, 32, 128)][:(4 if SMALL else None)]:
-            try:
-                qkv = torch.randn(B * S, (H + 2 * KVH) * hd, device=dev).bfloat16()
-                do = torch.randn(B * S, H * hd, device=dev).bfloat16()
-                sc = hd ** -0.5
-                r = dict(B=B, S=S, H=H, KVH=KVH, hd=hd, fwd_version=ver, bwd_version=bver)
-                o1, l1 = CK.attn_fwd(qkv, B, S, H, KVH, hd, sc)
-                torch.cuda.synchronize()
-                if S <= 1024:
-                    o0, l0 = TK.attn_fwd(qkv, B, S, H, KVH, hd, sc)
-                    r.update(o=relerr(o1, o0), lse=relerr(l1, l0))
-                    g1 = CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, sc)
-                    g0 = TK.attn_bwd(do, qkv, o0, l0, B, S, H, KVH, hd, sc)
-                    r.update(dqkv=relerr(g1, g0))
-                else:
-                    o0 = CK._sdpa_fwd(qkv, B, S, H, KVH, hd, sc)
-                    r.update(o_vs_sdpa=relerr(o1, o0))
-                    fl = 4 * B * H * S * S * hd / 2
-                    ms = time_ms(lambda: CK.attn_fwd(qkv, B, S, H, KVH, hd, sc))
-                    ms0 = time_ms(lambda: CK._sdpa_fwd(qkv, B, S, H, KVH, hd, sc))
-                    r.update(fwd_ms=ms, fwd_tflops=fl / ms / 1e9, sdpa_fwd_ms=ms0, sdpa_fwd_tflops=fl / ms0 / 1e9)
-                    ms = time_ms(lambda: CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, sc))
-                    r.update(bwd_ms=ms, bwd_tflops=2.5 * fl / ms / 1e9)
-                rec("attn", **r)
-            except Exception as ex:
-                rec("attn", B=B, S=S, H=H, KVH=KVH, hd=hd, ok=False, error=repr(ex)[:500])
+        for (B, S, H, KVH, hd) in [(1, 128, 1, 1, 128), (2, 256, 4, 2, 128), (1, 384, 2, 1, 128), (1, 512, 2, 2, 64), (2, 4096, 32, 32, 128)][:(4 if SMALL else None)]:
+          try:
+              qkv = torch.randn(B * S, (H + 2 * KVH) * hd, device=dev).bfloat16()
+              do = torch.randn(B * S, H * hd, device=dev).bfloat16()
+              sc = hd ** -0.5
+              r = dict(B=B, S=S, H=H, KVH=KVH, hd=hd)
+              o1, l1 = CK.attn_fwd(qkv, B, S, H, KVH, hd, sc)
+              torch.cuda.synchronize()
+              if S <= 1024:
+                  o0, l0 = TK.attn_fwd(qkv, B, S, H, KVH, hd, sc)
+                  r.update(o=relerr(o1, o0), lse=relerr(l1, l0))
+                  g1 = CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, sc)
+                  g0 = TK.attn_bwd(do, qkv, o0, l0, B, S, H, KVH, hd, sc)
+                  r.update(dqkv=relerr(g1, g0))
+              else:
+                  o0 = CK._sdpa_fwd(qkv, B, S, H, KVH, hd, sc)
+                  r.update(o_vs_sdpa=relerr(o1, o0))
+                  fl = 4 * B * H * S * S * hd / 2
+                  ms = time_ms(lambda: CK.attn_fwd(qkv, B, S, H, KVH, hd, sc))
+                  ms0 = time_ms(lambda: CK._sdpa_fwd(qkv, B, S, H, KVH, hd, sc))
+                  r.update(fwd_ms=ms, fwd_tflops=fl / ms / 1e9, sdpa_fwd_ms=ms0, sdpa_fwd_tflops=fl / ms0 / 1e9)
+                  ms = time_ms(lambda: CK.attn_bwd(do, qkv, o1, l1, B, S, H, KVH, hd, sc))
+                  r.update(bwd_ms=ms, bwd_tflops=2.5 * fl / ms / 1e9)
+              rec("attn", **r)
+          except Exception as ex:
+              rec("attn", B=B, S=S, H=H, KVH=KVH, hd=hd, ok=False, error=repr(ex)[:500])
 
     rec("done", launches=CK.launch_count())
 

@@ -73,7 +73,7 @@ def test_wgrad_uses_output_size_and_leftover_is_flushed(rec):
 def test_ineligible_gemm_leaves_prefetch_queued_but_flushes_dependent(rec):
     req = _req(0, 4 * 65536)
     ck.push_ag_request(req)
-    small = _meta(64, 128)                                                 # M < 256: not a CTA-pair GEMM
+    small = _meta(64, 128)                                                 # M < 256: not a fused-epilogue GEMM
     assert not ck._try_fused_gather(small, _meta(256, 128), "nt", _meta(64, 256), 0, None)
     assert ck._AG_QUEUE == [req] and not rec.ag and not rec.plain
 

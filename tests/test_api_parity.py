@@ -1,13 +1,14 @@
-"""Every public top-level name (and public method) of the reference's modules must exist under the same import path
-(`fms_fsdp.*` aliases to `fms_fsdp_b200.*`).  The reference tree is read-only input at /root/reference; the test is
-skipped when it is not mounted (e.g. in CI)."""
-import ast
+"""Every public top-level name (and public method) of the original project's modules must exist under the same import
+path (`fms_fsdp.*` aliases to `fms_fsdp_b200.*`).  The original names and parameter lists are recorded in
+tests/golden/reference_api.json.gz (oracle/make_golden.py)."""
+import gzip
 import importlib
+import json
 import os
 
 import pytest
 
-REF = "/root/reference"
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_api.json.gz")
 MODULES = {
     "fms_fsdp/config/training.py": "fms_fsdp.config.training",
     "fms_fsdp/utils/config_utils.py": "fms_fsdp.utils.config_utils",
@@ -28,23 +29,21 @@ MODULES = {
 }
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not mounted")
+def _recorded(path):
+    with gzip.open(GOLDEN, "rt") as f:
+        return json.load(f)[path]
+
+
 @pytest.mark.parametrize("path,mod", sorted(MODULES.items()))
 def test_public_names_of_reference_module_exist(path, mod):
-    tree = ast.parse(open(os.path.join(REF, path)).read())
+    rec = _recorded(path)
     ours = importlib.import_module(mod)
-    missing = []
-    for node in tree.body:
-        if isinstance(node, (ast.FunctionDef, ast.ClassDef)) and not node.name.startswith("_"):
-            if not hasattr(ours, node.name):
-                missing.append(node.name)
-            elif isinstance(node, ast.ClassDef):
-                cls = getattr(ours, node.name)
-                missing += [f"{node.name}.{b.name}" for b in node.body
-                            if isinstance(b, ast.FunctionDef) and not b.name.startswith("_") and not hasattr(cls, b.name)]
-        elif isinstance(node, ast.Assign):
-            missing += [t.id for t in node.targets
-                        if isinstance(t, ast.Name) and not t.id.startswith("_") and not hasattr(ours, t.id)]
+    missing = [n for n in rec["names"] if not hasattr(ours, n)]
+    for cname, methods in rec["classes"].items():
+        if cname.startswith("_") or not hasattr(ours, cname):
+            continue
+        cls = getattr(ours, cname)
+        missing += [f"{cname}.{m}" for m in methods if not m.startswith("_") and not hasattr(cls, m)]
     assert not missing, f"{mod} lacks {missing}"
 
 
@@ -53,17 +52,16 @@ def _positional_names(fn_node):
     return [x.arg for x in a.posonlyargs + a.args if x.arg not in ("self", "cls")], [x.arg for x in a.kwonlyargs]
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree not mounted")
 @pytest.mark.parametrize("path,mod", sorted(MODULES.items()))
 def test_signatures_accept_the_reference_call_forms(path, mod):
     """Every public function / method (and ``__init__``) takes the reference's parameters under the same names and, unless it
     takes ``*args``, at the same positions -- so both keyword and positional call sites of reference users keep working."""
     import inspect
-    tree = ast.parse(open(os.path.join(REF, path)).read())
+    rec = _recorded(path)
     ours = importlib.import_module(mod)
     problems = []
 
-    def check(node, obj, label):
+    def check(recorded, obj, label):
         try:
             params = list(inspect.signature(obj).parameters.values())
         except (TypeError, ValueError):
@@ -71,7 +69,7 @@ def test_signatures_accept_the_reference_call_forms(path, mod):
         names = [p.name for p in params if p.name not in ("self", "cls")]
         var_kw = any(p.kind == p.VAR_KEYWORD for p in params)
         var_pos = any(p.kind == p.VAR_POSITIONAL for p in params)
-        pos, kwonly = _positional_names(node)
+        pos, kwonly = recorded
         for i, n in enumerate(pos):
             if n not in names:
                 if not var_kw:
@@ -80,12 +78,13 @@ def test_signatures_accept_the_reference_call_forms(path, mod):
                 problems.append(f"{label}: {n} is parameter {names.index(n)}, reference has it at {i}")
         problems.extend(f"{label}: no keyword {n}" for n in kwonly if n not in names and not var_kw)
 
-    for node in tree.body:
-        if isinstance(node, ast.FunctionDef) and not node.name.startswith("_") and hasattr(ours, node.name):
-            check(node, getattr(ours, node.name), node.name)
-        elif isinstance(node, ast.ClassDef) and hasattr(ours, node.name):
-            cls = getattr(ours, node.name)
-            for b in node.body:
-                if isinstance(b, ast.FunctionDef) and (b.name == "__init__" or not b.name.startswith("_")) and hasattr(cls, b.name):
-                    check(b, getattr(cls, b.name), f"{node.name}.{b.name}")
+    for name, sig in rec["functions"].items():
+        if hasattr(ours, name):
+            check(sig, getattr(ours, name), name)
+    for cname, methods in rec["classes"].items():
+        if hasattr(ours, cname):
+            cls = getattr(ours, cname)
+            for m, sig in methods.items():
+                if hasattr(cls, m):
+                    check(sig, getattr(cls, m), f"{cname}.{m}")
     assert not problems, f"{mod}: {problems}"

@@ -284,21 +284,22 @@ def test_dummy_loader_and_causal_lm():
     assert parse_data_args("a,b", "1,2.5") == (["a", "b"], [1.0, 2.5])
 
 
-# ------------------------------------------------------------------- interchange with the unmodified reference
-_REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
+# ------------------------------------------------------------------- interchange with the original project
+# The original dataset classes were run once on the corpora below (oracle/make_golden.py); tests/golden holds what they
+# yielded and the loader checkpoints they wrote, so these tests need nothing outside the repository.
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
-def _reference_dataset_module():
-    """The reference's own ``fms_fsdp.utils.dataset_utils`` from the offline install under baseline/_ref (DESIGN.md §4),
-    loaded under a private name so it cannot shadow this repo's ``fms_fsdp`` alias package."""
-    import importlib.util
-    path = os.path.join(_REF, "fms_fsdp", "utils", "dataset_utils.py")
-    if not os.path.exists(path):
-        pytest.skip("reference install (baseline/_ref) not present")
-    spec = importlib.util.spec_from_file_location("_reference_dataset_utils", path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+@pytest.fixture(scope="module")
+def golden():
+    import gzip
+    import json
+    with gzip.open(os.path.join(GOLDEN, "reference_datasets.json.gz"), "rt") as f:
+        return json.load(f)
+
+
+def lines(it, n):
+    return [list(map(int, next(it))) for _ in range(n)]
 
 
 def _full_stack(D, corpus, rank, world, seq=33):
@@ -309,34 +310,39 @@ def _full_stack(D, corpus, rank, world, seq=33):
     return D.PreloadBufferDataset(d, 50)
 
 
-def test_token_stream_and_loader_checkpoints_interchange_with_the_reference(corpus, tmp_path):
-    """Same corpus, same pipeline, both implementations: (1) the token streams are identical line by line; (2) a loader
-    checkpoint written by this repo is resumed by the reference's classes, and one written by the reference is resumed here
-    -- also across a change of world size (2 -> 4 ranks) -- and both continuations agree."""
+def _copy_ckpt(name, dst):
+    import shutil
+    shutil.copytree(os.path.join(GOLDEN, "reference_ckpt", name), dst)
+    return str(dst)
+
+
+def test_token_stream_and_loader_checkpoints_interchange_with_the_reference(corpus, tmp_path, golden):
+    """Same corpus, same pipeline: (1) the token stream is the original project's line by line; (2) a loader checkpoint
+    written here (world 2) continues in the original classes exactly as it continues here, and one the original classes
+    wrote (world 2) is resumed here at world 4 exactly as the original classes resume it."""
     import fms_fsdp_b200.utils.dataset_utils as OURS
-    REF = _reference_dataset_module()
 
-    a, b = iter(_full_stack(OURS, corpus, 0, 1)), iter(_full_stack(REF, corpus, 0, 1))
-    for _ in range(300):
-        assert list(next(a)) == list(next(b))
+    assert lines(iter(_full_stack(OURS, corpus, 0, 1)), 300) == golden["full_stack"]
 
-    # (2a) ours writes at world 2, the reference resumes at world 2; (2b) the reference writes, we resume at world 4
-    for writer, reader, new_world, tag in ((OURS, REF, 2, "ours_to_ref"), (REF, OURS, 4, "ref_to_ours")):
-        ck = str(tmp_path / tag)
-        stacks = [_full_stack(writer, corpus, r, 2) for r in range(2)]
-        its = [iter(s) for s in stacks]
-        for it in its:
-            take(it, 40)
-        for s in stacks:
-            s.save_to_path(ck)
-        resumed_other = [_full_stack(reader, corpus, r, new_world) for r in range(new_world)]
-        resumed_same = [_full_stack(writer, corpus, r, new_world) for r in range(new_world)]
-        for s in resumed_other + resumed_same:
-            s.load_from_path(ck)
-        for x, y in zip(resumed_other, resumed_same):
-            ix, iy = iter(x), iter(y)
-            for _ in range(60):
-                assert list(next(ix)) == list(next(iy)), tag
+    # (2a) ours writes at world 2; the original classes' continuation at world 2 was recorded from such a checkpoint
+    ck = str(tmp_path / "ours_to_ref")
+    stacks = [_full_stack(OURS, corpus, r, 2) for r in range(2)]
+    for s in stacks:
+        take(iter(s), 40)
+    for s in stacks:
+        s.save_to_path(ck)
+    resumed = [_full_stack(OURS, corpus, r, 2) for r in range(2)]
+    for s in resumed:
+        s.load_from_path(ck)
+    assert [lines(iter(s), 60) for s in resumed] == golden["ours_to_ref"]
+
+    # (2b) the original classes wrote at world 2; resumed here at world 4, every rank continues with the lines the
+    # original classes continued with from the same checkpoint
+    ref_ck = _copy_ckpt("full_stack_w2", tmp_path / "ref_to_ours")
+    for r in range(4):
+        x = _full_stack(OURS, corpus, r, 4)
+        x.load_from_path(ref_ck)
+        assert lines(iter(x), 60) == golden["ref_w2_to_w4"][r], r
 
 
 # ------------------------------------------------------------------------ parquet / auto handlers (raw text + tokenizer)
@@ -361,7 +367,7 @@ def text_corpus():
     return tmp, docs, vocab
 
 
-def test_parquet_and_auto_handlers_tokenise_strip_and_match_the_reference(text_corpus):
+def test_parquet_and_auto_handlers_tokenise_strip_and_match_the_reference(text_corpus, golden):
     from fms_fsdp_b200.utils.dataset_utils import AutoHandler, ParquetHandler
     tmp, docs, vocab = text_corpus
     h = ParquetHandler(f"{tmp}/tok", "text")
@@ -380,15 +386,10 @@ def test_parquet_and_auto_handlers_tokenise_strip_and_match_the_reference(text_c
     r = a.open(path)
     assert a.get(r, 0, {1, 2}) == [vocab[w] for w in docs[0].split()]
 
-    # the whole reader on the mixed folder: same documents, same order as the unmodified reference classes
-    REF = _reference_dataset_module()
+    # the whole reader on the mixed folder: same documents, same order as the original classes
     ours = StreamingDocDataset(f"{tmp}/data/mix", 0, 1, AutoHandler(f"{tmp}/tok", "text"), 0, strip_tokens={1, 2}, seed=3,
                                max_chunksize=16)
-    theirs = REF.StreamingDocDataset(f"{tmp}/data/mix", 0, 1, REF.AutoHandler(f"{tmp}/tok", "text"), 0, strip_tokens={1, 2},
-                                     seed=3, max_chunksize=16)
-    io, it = iter(ours), iter(theirs)
-    for _ in range(200):
-        assert list(next(io)) == list(next(it))
+    assert lines(iter(ours), 200) == golden["auto_reader"]
 
 
 def test_get_data_loader_with_file_type_auto_runs_on_text_and_token_shards(text_corpus, tmp_path):
@@ -411,98 +412,90 @@ def test_get_data_loader_with_file_type_auto_runs_on_text_and_token_shards(text_
     assert any(10 <= t < 210 for t in seen) and any(t >= 300 for t in seen)   # both the text and the token shard are read
 
 
-@pytest.mark.parametrize("kw", [dict(pack_hard=False, pad_token=-5), dict(pack_hard=False, pad_token=-5, bos_token=-2, eos_token=-3),
-                                dict(pack_hard=True, bos_token=-2), dict(pack_hard=True, eos_token=-3, bos_token=-2)])
-def test_line_packer_modes_equal_the_reference(corpus, kw):
-    """Every packing mode of ``BufferDataset`` (hard / soft packing, per-line BOS / EOS, padding) against the unmodified
-    reference class on the same sampled two-dataset stream."""
-    import fms_fsdp_b200.utils.dataset_utils as OURS
-    REF = _reference_dataset_module()
-
-    def build(D):
-        d = D.StreamingDocDataset(corpus, 0, 1, D.ArrowHandler(), -1, seed=11, max_chunksize=40)
-        d = D.SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[1, 2], verbose=False)
-        return D.BufferDataset(d, 37, **kw)
-
-    a, b = iter(build(OURS)), iter(build(REF))
-    for _ in range(250):
-        assert list(next(a)) == list(next(b))
+PACKER_MODES = [dict(pack_hard=False, pad_token=-5), dict(pack_hard=False, pad_token=-5, bos_token=-2, eos_token=-3),
+                dict(pack_hard=True, bos_token=-2), dict(pack_hard=True, eos_token=-3, bos_token=-2)]
 
 
-@pytest.mark.parametrize("world,rank,bos,min_len,nlog", [(3, 1, None, 1, 6), (2, 0, -9, 3, 8), (4, 3, -9, 60, 12), (1, 0, None, 101, 5)])
-def test_reader_partitioning_options_equal_the_reference(corpus, world, rank, bos, min_len, nlog):
+@pytest.mark.parametrize("mode", range(len(PACKER_MODES)))
+def test_line_packer_modes_equal_the_reference(corpus, golden, mode):
+    """Every packing mode of ``BufferDataset`` (hard / soft packing, per-line BOS / EOS, padding) against the original
+    class on the same sampled two-dataset stream."""
+    d = StreamingDocDataset(corpus, 0, 1, ArrowHandler(), -1, seed=11, max_chunksize=40)
+    d = SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[1, 2], verbose=False)
+    assert lines(iter(BufferDataset(d, 37, **PACKER_MODES[mode])), 250) == golden["line_packer"][mode]
+
+
+PARTITION_CASES = [(3, 1, None, 1, 6), (2, 0, -9, 3, 8), (4, 3, -9, 60, 12), (1, 0, None, 101, 5)]
+
+
+@pytest.mark.parametrize("world,rank,bos,min_len,nlog", PARTITION_CASES)
+def test_reader_partitioning_options_equal_the_reference(corpus, golden, world, rank, bos, min_len, nlog):
     """Document reader + logical shards under different partitionings, BOS insertion and minimum document lengths (which
-    drop all of dataset_2's 50-token documents at 60 and everything at 101): chunk for chunk what the reference yields."""
+    drop all of dataset_2's 50-token documents at 60 and everything at 101): chunk for chunk what the original yields."""
     # (50 tokens + delimiter + BOS = 52 < 60)
-    import fms_fsdp_b200.utils.dataset_utils as OURS
-    REF = _reference_dataset_module()
-
-    def build(D):
-        d = D.StreamingDocDataset(os.path.join(corpus, "dataset_2") if min_len < 101 else corpus, rank, world, D.ArrowHandler(),
-                                  -1, bos_token=bos, min_length=min_len, seed=5, max_chunksize=33)
-        return D.ScalableShardDataset(d, -1, n_logical_shards=nlog * world)
-
+    d = StreamingDocDataset(os.path.join(corpus, "dataset_2") if min_len < 101 else corpus, rank, world, ArrowHandler(),
+                            -1, bos_token=bos, min_length=min_len, seed=5, max_chunksize=33)
+    d = ScalableShardDataset(d, -1, n_logical_shards=nlog * world)
     if min_len >= 60:
-        # nothing survives the length filter: the reference spins forever in that case; here it is an error that says why
+        # nothing survives the length filter: the original spins forever in that case; here it is an error that says why
         with pytest.raises(RuntimeError, match="min_length"):
-            next(iter(build(OURS)))
+            next(iter(d))
         return
-    a, b = iter(build(OURS)), iter(build(REF))
-    for _ in range(150):
-        assert list(next(a)) == list(next(b))
+    assert lines(iter(d), 150) == golden["partitioning"][f"{world},{rank},{bos},{min_len},{nlog}"]
 
 
-@pytest.mark.parametrize("writer_is_ours,old_world,new_world", [(True, 3, 2), (False, 4, 6), (True, 6, 4), (False, 2, 1)])
-def test_rescaled_resume_equals_the_reference_for_more_world_size_pairs(corpus, tmp_path, writer_is_ours, old_world, new_world):
-    """Loader checkpoints written at ``old_world`` ranks by one implementation, resumed at ``new_world`` ranks by both: every
-    new rank continues with the same lines in either implementation (shrinking, growing, non-divisible pairs)."""
+RESCALE_CASES = [(True, 3, 2), (False, 4, 6), (True, 6, 4), (False, 2, 1)]
+
+
+def _rescale_stack(D, corpus, rank, world):
+    d = D.StreamingDocDataset(corpus, rank, world, D.ArrowHandler(), -1, strip_tokens={-1}, min_length=3, seed=7)
+    d = D.ScalableShardDataset(d, -1, n_logical_shards=12)
+    d = D.SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[3, 1], verbose=False)
+    d = D.BufferDataset(d, 33, bos_token=None, eos_token=None, pack_hard=True)
+    return D.PreloadBufferDataset(d, 50)
+
+
+@pytest.mark.parametrize("writer_is_ours,old_world,new_world", RESCALE_CASES)
+def test_rescaled_resume_equals_the_reference_for_more_world_size_pairs(corpus, tmp_path, golden, writer_is_ours, old_world,
+                                                                         new_world):
+    """Loader checkpoints written at ``old_world`` ranks by one implementation (here, or the original classes: their
+    checkpoint is stored), resumed at ``new_world`` ranks: every new rank continues with the lines the original classes
+    continued with (shrinking, growing, non-divisible pairs)."""
     import fms_fsdp_b200.utils.dataset_utils as OURS
-    REF = _reference_dataset_module()
-    writer = OURS if writer_is_ours else REF
-    ck = str(tmp_path / "ck")
-
-    def stack(D, rank, world):
-        d = D.StreamingDocDataset(corpus, rank, world, D.ArrowHandler(), -1, strip_tokens={-1}, min_length=3, seed=7)
-        d = D.ScalableShardDataset(d, -1, n_logical_shards=12)
-        d = D.SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[3, 1], verbose=False)
-        d = D.BufferDataset(d, 33, bos_token=None, eos_token=None, pack_hard=True)
-        return D.PreloadBufferDataset(d, 50)
-
-    olds = [stack(writer, r, old_world) for r in range(old_world)]
-    for s in olds:
-        take(iter(s), 30)
-    for s in olds:
-        s.save_to_path(ck)
+    if writer_is_ours:
+        ck = str(tmp_path / "ck")
+        olds = [_rescale_stack(OURS, corpus, r, old_world) for r in range(old_world)]
+        for s in olds:
+            take(iter(s), 30)
+        for s in olds:
+            s.save_to_path(ck)
+    else:
+        ck = _copy_ckpt(f"rescale_{old_world}", tmp_path / "ck")
+    want = golden["rescaled"][f"{int(writer_is_ours)},{old_world},{new_world}"]
     for r in range(new_world):
-        a, b = stack(OURS, r, new_world), stack(REF, r, new_world)
-        a.load_from_path(ck); b.load_from_path(ck)
-        ia, ib = iter(a), iter(b)
-        for _ in range(40):
-            assert list(next(ia)) == list(next(ib)), (r, new_world)
+        a = _rescale_stack(OURS, corpus, r, new_world)
+        a.load_from_path(ck)
+        assert lines(iter(a), 40) == want[r], (r, new_world)
 
 
-def test_multi_worker_dataloader_stream_equals_the_reference(corpus, tmp_path):
+def _worker_loader(D, corpus, path):
+    d = D.StreamingDocDataset(corpus, 1, 2, D.ArrowHandler(), -1, min_length=3, seed=3)
+    d = D.ScalableShardDataset(d, -1, n_logical_shards=8)
+    d = D.SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[1, 1], verbose=False)
+    d = D.BufferDataset(d, 21, pack_hard=True)
+    d = D.PreloadBufferDataset(d, 20)
+    d = D.PreprocessDataset(d, torch.IntTensor)
+    d = D.CheckpointDataset(d, path, 5, 2, path)
+    return torch.utils.data.DataLoader(d, num_workers=2, batch_size=2)
+
+
+def test_multi_worker_dataloader_stream_equals_the_reference(corpus, tmp_path, golden):
     """Through ``torch.utils.data.DataLoader(num_workers=2)``: each worker process derives its own partition from
-    (rank, world, worker id); the batches of both implementations are identical, including the in-worker auto-checkpoints."""
+    (rank, world, worker id); the batches equal the original project's, including the in-worker auto-checkpoints."""
     import fms_fsdp_b200.utils.dataset_utils as OURS
-    REF = _reference_dataset_module()
-
-    def loader(D, tag):
-        d = D.StreamingDocDataset(corpus, 1, 2, D.ArrowHandler(), -1, min_length=3, seed=3)
-        d = D.ScalableShardDataset(d, -1, n_logical_shards=8)
-        d = D.SamplingDataset(corpus, d, -1, datasets=["dataset_1", "dataset_2"], weights=[1, 1], verbose=False)
-        d = D.BufferDataset(d, 21, pack_hard=True)
-        d = D.PreloadBufferDataset(d, 20)
-        d = D.PreprocessDataset(d, torch.IntTensor)
-        d = D.CheckpointDataset(d, str(tmp_path / tag), 5, 2, str(tmp_path / tag))
-        return torch.utils.data.DataLoader(d, num_workers=2, batch_size=2)
-
-    a, b = iter(loader(OURS, "ours")), iter(loader(REF, "ref"))
-    for _ in range(24):
-        assert torch.equal(next(a), next(b))
-    del a, b
+    a = iter(_worker_loader(OURS, corpus, str(tmp_path / "ours")))
+    assert [next(a).tolist() for _ in range(24)] == golden["multi_worker"]
+    del a
     mine = sorted(os.listdir(tmp_path / "ours" / "checkpoints"))
-    theirs = sorted(os.listdir(tmp_path / "ref" / "checkpoints"))
-    assert mine == theirs and mine, (mine, theirs)
-    step_dir = mine[-1]
-    assert sorted(os.listdir(tmp_path / "ours" / "checkpoints" / step_dir)) == sorted(os.listdir(tmp_path / "ref" / "checkpoints" / step_dir))
+    assert mine and mine == golden["multi_worker_ckpts"]["steps"]
+    assert sorted(os.listdir(tmp_path / "ours" / "checkpoints" / mine[-1])) == golden["multi_worker_ckpts"]["last"]

@@ -130,7 +130,7 @@ def test_signal_post_wait_and_scalar_allreduce(C):
 @pytest.mark.parametrize("W", [2, 8])
 @pytest.mark.parametrize("dependent", [True, False])
 def test_ag_gemm_gathers_from_pointer_table(C, W, dependent):
-    """All-gather fused into the CTA-pair GEMM: the comm warps pull W 'peer' shards into the gathered buffer; in
+    """All-gather fused into the GEMM: the comm warps pull W 'peer' shards into the gathered buffer; in
     dependent mode the GEMM's own B operand is that buffer, consumed tile by tile behind the ready flags."""
     from fms_fsdp_b200.ops import cuda_kernels as CK
     torch.manual_seed(5)

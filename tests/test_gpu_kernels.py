@@ -1,4 +1,4 @@
-"""GPU tier (run on the B200 box with ``pytest -m gpu``): every sm_100a kernel against the plain-PyTorch
+"""GPU tier (run on an H100 with ``pytest -m gpu``): every sm_90a kernel against the plain-PyTorch
 fp32 oracle of the same op (``ops/torch_kernels.py``), and the engine on the fused kernels against the ATen
 kernel path.  These tests load ``fms_fsdp_b200/_C.so`` -- there is no silent eager fallback."""
 import os
@@ -148,7 +148,7 @@ def test_conv1d(K):
 
 
 def test_engine_fused_kernels_match_aten_path():
-    """Same model + data: sm_100a kernel path vs ATen path (bf16), loss trajectory and grad norms agree."""
+    """Same model + data: sm_90a kernel path vs ATen path (bf16), loss trajectory and grad norms agree."""
     from fms_fsdp_b200.models.llama import LLaMA, LLaMAConfig
     from fms_fsdp_b200.ops import cuda_kernels as CK
     from fms_fsdp_b200.ops import set_kernel_path
@@ -188,26 +188,26 @@ def test_smoke_entry():
     g.smoke()
 
 
-if torch.cuda.device_count() >= 2:
-    # Real NVLink run (2 ranks).  On the 1-GPU test box the same kernels are exercised through local pointer tables in
-    # tests/test_gpu_collectives_1gpu.py, so this test only EXISTS where it can run (nothing is skipped on 1 GPU).
-    def test_fused_collectives_two_gpus():
-        env = dict(os.environ, PYTHONPATH=ROOT)
-        r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
-                            "--master-addr", "127.0.0.1", "--master-port", "29541",
-                            os.path.join(ROOT, "scripts", "gpu_multi_check.py"), "all"],
-                           env=env, capture_output=True, text=True, timeout=600, cwd=ROOT)
-        assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
-        import json
-        out = json.load(open(os.path.join(ROOT, "gpurun_out", "multi_2.json")))
-        assert out["allgather_equal"] and out["reduce_scatter_maxdiff"] < 1e-3
-        f, t = out["engine_fsdp"]["fused"], out["engine_fsdp"]["torch"]
-        assert all(abs(a[1] - b[1]) < 2e-2 * b[1] for a, b in zip(f, t))
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs with peer access")
+def test_fused_collectives_two_gpus():
+    """Real NVLink run (2 ranks).  On one GPU the same kernels are exercised through local pointer tables in
+    tests/test_gpu_collectives_1gpu.py."""
+    env = dict(os.environ, PYTHONPATH=ROOT)
+    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2",
+                        "--master-addr", "127.0.0.1", "--master-port", "29541",
+                        os.path.join(ROOT, "scripts", "gpu_multi_check.py"), "all"],
+                       env=env, capture_output=True, text=True, timeout=600, cwd=ROOT)
+    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-2000:]
+    import json
+    out = json.load(open(os.path.join(ROOT, "gpurun_out", "multi_2.json")))
+    assert out["allgather_equal"] and out["reduce_scatter_maxdiff"] < 1e-3
+    f, t = out["engine_fsdp"]["fused"], out["engine_fsdp"]["torch"]
+    assert all(abs(a[1] - b[1]) < 2e-2 * b[1] for a, b in zip(f, t))
 
 
 @pytest.mark.parametrize("shape", [(2, 256, 8, 64, 1, 128), (1, 384, 8, 64, 2, 64)])
 def test_ssd_scan_native_vs_chunked_oracle(K, shape):
-    """Mamba2 SSD scan: batched tcgen05 GEMMs + csrc/ssd.cu glue against the fp32 ATen chunked formulation."""
+    """Mamba2 SSD scan: batched wgmma GEMMs + csrc/ssd.cu glue against the fp32 ATen chunked formulation."""
     CK, TK = K
     Bs, S, H, P, G, N = shape
     M = Bs * S
@@ -260,7 +260,7 @@ def test_selective_scan_native_vs_sequential_oracle(K, use_z):
 
 
 def test_qkv_attention_rope_fused_in_gemm_and_bwd_epilogues(K):
-    """RoPE as the epilogue of the CTA-pair QKV GEMM (forward) and of the dq/dk kernels (backward) against the
+    """RoPE as the epilogue of the QKV GEMM (forward) and of the dq/dk kernels (backward) against the
     unfused CUDA path (GEMM, in-place RoPE kernel, attention) and its autograd."""
     from fms_fsdp_b200 import ops
     CK, TK = K
@@ -324,7 +324,7 @@ def test_gated_mlp_node_matches_unfused_ops(K):
 
 
 def test_fp8_rowwise_quant_and_e4m3_gemm(K):
-    """Opt-in fp8 forward path: row-wise e4m3 quantisation kernel and the kind::f8f6f4 CTA-pair GEMM against the torch
+    """Opt-in fp8 forward path: row-wise e4m3 quantisation kernel and the e4m3 wgmma GEMM against the torch
     float8_e4m3fn oracle (the GEMM is exact on the quantised values up to fp32 summation order and bf16 rounding)."""
     CK, TK = K
     torch.manual_seed(4)

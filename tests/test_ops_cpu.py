@@ -1,5 +1,5 @@
 """Hand-derived backward formulas of every op (ATen back-end) against autograd of the naive formula.
-The same primitives are what the sm_100a kernels are checked against on the GPU box."""
+The same primitives are what the sm_90a kernels are checked against on the GPU box."""
 import torch
 import torch.nn.functional as F
 

@@ -1,7 +1,6 @@
-"""The shipped extension is Blackwell-native: every tensor-core instruction in it is a tcgen05 MMA (SASS ``UTCHMMA`` /
-``UTCQMMA``), operands arrive by TMA (``UTMALDG``), accumulators are read from TMEM (``LDTM``), the pushing wgrad GEMM stores
-with bulk copies (``UBLKCP``) -- and there is not a single legacy warp-level ``HMMA`` (``mma.sync`` / ``wmma``) in the binary.
-Runs wherever ``cuobjdump`` and the built ``_C.so`` exist (no GPU needed)."""
+"""The shipped extension is Hopper-native: every tensor-core instruction in it is a warpgroup MMA (SASS ``HGMMA`` /
+``QGMMA``, from ``wgmma.mma_async``), operands arrive by TMA (``UTMALDG``) -- and there is not a single legacy warp-level
+``HMMA`` (``mma.sync`` / ``wmma``) in the binary.  Runs wherever ``cuobjdump`` and the built ``_C.so`` exist (no GPU needed)."""
 import os
 import re
 import shutil
@@ -19,7 +18,8 @@ def kernels():
     if not os.path.exists(SO) or not os.path.exists(exe):
         pytest.skip("needs the built extension and cuobjdump")
     out = subprocess.run([exe, "-sass", SO], capture_output=True, text=True, timeout=600).stdout
-    assert "arch = sm_100a" in out
+    assert "arch = sm_90a" in out
+    assert not re.search(r"arch = sm_(?!90a)", out)
     per = {}
     name = None
     for line in out.splitlines():
@@ -44,22 +44,24 @@ def _has(kernels, name_part, *mnemonics):
 def test_no_legacy_warp_level_mma_anywhere(kernels):
     legacy = [k for k, body in kernels.items() if re.search(r"(?<![A-Z])HMMA\.|(?<![A-Z])IMMA\.|(?<![A-Z])QMMA\.", body)]
     assert not legacy, legacy[:5]
-    assert sum("UTCHMMA" in b or "UTCQMMA" in b for b in kernels.values()) >= 40     # GEMM + attention instantiations
+    assert sum("HGMMA" in b or "QGMMA" in b for b in kernels.values()) >= 40     # GEMM + attention instantiations
 
 
-def test_hot_kernels_use_tcgen05_tma_tmem(kernels):
-    gemm = _has(kernels, "gemm2_bf16_tcgen05", r"UTCHMMA\.2CTA|UTCQMMA\.2CTA", r"UTMALDG\.2D", r"LDTM")
+def test_hot_kernels_use_wgmma_and_tma(kernels):
+    gemm = _has(kernels, "gemm_bf16_wgmma", r"HGMMA\.64x128x16|QGMMA\.64x128x32", r"UTMALDG\.[24]D", r"WARPGROUP\.ARRIVE")
     assert len(gemm) >= 20
-    _has(kernels, "attn_fwd2_kernel", r"UTCHMMA", r"UTMALDG", r"LDTM", r"MUFU\.EX2")
-    _has(kernels, "attn_bwd3_kernel", r"UTCHMMA", r"UTMALDG", r"LDTM", r"STTM")
-    # fp8 instantiation: kind::f8f6f4 on the CTA pair
-    assert any("UTCQMMA.2CTA" in b for k, b in kernels.items() if "gemm2_bf16_tcgen05" in k)
+    _has(kernels, "attn_fwd_kernel", r"HGMMA\.64x128x16", r"UTMALDG", r"MUFU\.EX2")
+    _has(kernels, "attn_bwd_kernel", r"HGMMA\.64x64x16", r"UTMALDG", r"MUFU\.EX2")
+    # fp8 instantiation: e4m3 warpgroup MMA
+    assert any("QGMMA.64x128x32.F32.E4M3.E4M3" in b for k, b in kernels.items() if "gemm_bf16_wgmma" in k)
 
 
 def test_push_epilogue_and_peer_collectives(kernels):
-    push = [k for k, b in kernels.items() if "gemm2_bf16_tcgen05" in k and "UBLKCP.G.S" in b]
-    assert len(push) >= 2                                   # wgrad push, with and without the fused all-gather
+    # EPI_PUSH = 4: wgrad push, with and without the fused all-gather
+    push = [k for k in kernels if "gemm_bf16_wgmma" in k and "ELi4E" in k]
+    assert len(push) >= 2
+    assert all("UBLKCP.G.S" in kernels[k] for k in push)     # staged rows leave as cp.async.bulk stores
     # comm warps of the all-gather GEMMs read peers with system-scope 16-byte loads
-    assert any("LDG.E.128.STRONG.SYS" in b for k, b in kernels.items() if "gemm2_bf16_tcgen05" in k)
+    assert any("LDG.E.128.STRONG.SYS" in b for k, b in kernels.items() if "gemm_bf16_wgmma" in k)
     _has(kernels, "signal_barrier_kernel", r"ST\S*\.STRONG\.SYS|STG\S*\.SYS", r"LD\S*\.STRONG\.SYS")
     _has(kernels, "reduce_scatter", r"LDG\.E\.128")

@@ -38,37 +38,21 @@ def test_non_reentrant_wrapper_marks_a_single_block():
     assert non_reentrant_wrapper(blk) is blk and is_checkpointed(blk)
 
 
+AC_FRACTIONS = ["1/7", "1/4", "1/3", "2/5", "1/2", "3/5", "2/3", "3/4", "9/10", "1"]
+AC_DEPTHS = [10, 24, 32, 40, 48, 80]
+
+
 def test_selection_equals_what_the_reference_install_wraps():
-    """Run the unmodified reference ``apply_fsdp_checkpointing`` (torch ``checkpoint_wrapper``) on stacks of plain blocks and
-    compare WHICH blocks it wrapped with ``selection_mask``, for the depths of the model zoo and a sweep of fractions."""
+    """The unmodified reference ``apply_fsdp_checkpointing`` (torch ``checkpoint_wrapper``) was run on stacks of plain
+    blocks for the depths of the model zoo and a sweep of fractions (oracle/make_golden.py); WHICH blocks it wrapped is
+    recorded in tests/golden and must equal ``selection_mask``."""
+    import gzip
     import json
     import os
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    ref = os.path.join(root, "baseline", "_ref")
-    if not os.path.exists(os.path.join(ref, "fms_fsdp", "policies", "ac_handler.py")):
-        pytest.skip("reference install (baseline/_ref) not present")
-    fracs = ["1/7", "1/4", "1/3", "2/5", "1/2", "3/5", "2/3", "3/4", "9/10", "1"]
-    depths = [10, 24, 32, 40, 48, 80]
-    code = (
-        "import sys, json\n"
-        f"sys.path = [{ref!r}] + [p for p in sys.path if p not in ('', {root!r})]\n"
-        "import importlib.util, torch.nn as nn\n"
-        f"spec = importlib.util.spec_from_file_location('ref_ac', {os.path.join(ref, 'fms_fsdp', 'policies', 'ac_handler.py')!r})\n"
-        "ac = importlib.util.module_from_spec(spec); spec.loader.exec_module(ac)\n"
-        "from torch.distributed.algorithms._checkpoint.checkpoint_wrapper import CheckpointWrapper\n"
-        "class Blk(nn.Linear):\n    pass\n"
-        "out = {}\n"
-        f"for n in {depths!r}:\n"
-        f"    for p in {fracs!r}:\n"
-        "        m = nn.Sequential(*[Blk(2, 2) for _ in range(n)])\n"
-        "        ac.apply_fsdp_checkpointing(m, Blk, p)\n"
-        "        out[f'{n}:{p}'] = [isinstance(c, CheckpointWrapper) for c in m]\n"
-        "print('OUT' + json.dumps(out))\n")
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd="/", timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
-    theirs = json.loads(r.stdout.split("OUT", 1)[1])
-    for n in depths:
-        for p in fracs:
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_selective_ac.json.gz")
+    with gzip.open(path, "rt") as f:
+        theirs = json.load(f)
+    assert sorted(theirs) == sorted(f"{n}:{p}" for n in AC_DEPTHS for p in AC_FRACTIONS)
+    for n in AC_DEPTHS:
+        for p in AC_FRACTIONS:
             assert selection_mask(n, p) == theirs[f"{n}:{p}"], (n, p)
