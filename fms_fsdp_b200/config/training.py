@@ -107,3 +107,4 @@ class train_config:
     loss_readback: bool = True               # every step: async 4-byte D2H of the loss into pinned memory, checked one step later
     poison_released_params: bool = False     # debug: NaN-fill a unit's gathered parameters on release (use-after-free trap)
     grad_dtype: str = "bf16"                 # dtype of the unsharded gradient buffer (reference reduce_dtype=bf16)
+    document_attention_mask: bool = False    # Llama: attention stops at eos_token in packed lines (RoPE positions are not reset)

@@ -13,6 +13,13 @@
 //            in registers (GQA group summed in the accumulator, no atomics);  dQ: CTA = (q tile 128, head, batch),
 //            streams (K_j, V_j) tiles of 64, dQ += dS K.  The score GEMMs are recomputed in both kernels in exchange
 //            for a deterministic, atomic-free dQ.
+//
+// Document masking (DOC = true, packed training rows): a segment table seg [2][B*S] int32 holds, per position, the
+// first (plane 0) and last (plane 1) position of its document within the row.  Key k is visible to query q when
+// seg0[q] <= k <= q, equivalently k <= q <= seg1[k].  Both planes are non-decreasing, so the first row of a q tile has
+// the smallest document start of the tile and the first row of a kv tile the smallest document end: whole tiles
+// outside the document band are skipped, the rest are masked per element like the diagonal.  Each kernel takes the
+// one plane it needs (forward and dQ: seg0; dK/dV: seg1), nullptr when DOC = false.
 #include "common.cuh"
 #include "tensormap.h"
 #include "wgmma.cuh"
@@ -56,10 +63,10 @@ struct FwdCfg {
   static constexpr int SMEM = TILE_BYTES * (1 + 2 + 2) + 1024 + 256;
 };
 
-template <int HD>
+template <int HD, bool DOC>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restrict__ o, float* __restrict__ lse,
-                int S, int H, int KVH, float scale_log2, int n_qt) {
+                int S, int H, int KVH, float scale_log2, int n_qt, const int* __restrict__ seg0) {
   using C = FwdCfg<HD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -76,9 +83,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
   const int kvh = h / (H / KVH);
   const int row0 = b * S + qt * 128;
   const int n_kv = min(qt + 1, (S + 127) / 128);
+  // DOC: kv tiles before the document of the tile's first row hold no visible key for any row of the tile
+  const int* srow = DOC ? seg0 + static_cast<size_t>(b) * S : nullptr;
+  const int j_lo = DOC ? srow[qt * 128] / 128 : 0;
 
   auto load_kv = [&](int j) {
-    const int st = j & 1;
+    const int st = (j - j_lo) & 1;
     const int krow = b * S + j * 128;
     mbar_arrive_expect_tx(&kv_full[st], 2 * C::TILE_BYTES);
     for (int c = 0; c < C::NCH; ++c) {
@@ -94,12 +104,18 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
     fence_barrier_init();
     mbar_arrive_expect_tx(q_full, C::TILE_BYTES);
     for (int c = 0; c < C::NCH; ++c) tma_load_2d(sQ + c * 16384, &tm, q_full, h * HD + 64 * c, row0);
-    for (int j = 0; j < 2 && j < n_kv; ++j) load_kv(j);
+    for (int j = j_lo; j < j_lo + 2 && j < n_kv; ++j) load_kv(j);
   }
   __syncthreads();
 
   const int r_lo = qt * 128 + wg * 64 + w4 * 16 + (lane >> 2);   // sequence index of the thread's rows r_lo, r_lo + 8
   const int cq = 2 * (lane & 3);
+  int doc_lo[2] = {0, 0}, tile_doc_hi = 0;     // DOC: document start of the thread's rows and of the tile's last row
+  if constexpr (DOC) {
+    doc_lo[0] = srow[min(r_lo, S - 1)];
+    doc_lo[1] = srow[min(r_lo + 8, S - 1)];
+    tile_doc_hi = srow[min(qt * 128 + 127, S - 1)];
+  }
   const uint64_t qd = make_smem_desc(smem_u32(sQ) + wg * 8192, 0, 1024);
   float oacc[HD / 2];
 #pragma unroll
@@ -107,9 +123,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
 
   mbar_wait(q_full, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j & 1;
-    mbar_wait(&kv_full[st], (j >> 1) & 1);
+  for (int j = j_lo; j < n_kv; ++j) {
+    const int st = (j - j_lo) & 1;
+    mbar_wait(&kv_full[st], ((j - j_lo) >> 1) & 1);
     const uint64_t kd = make_smem_desc(smem_u32(sK + st * C::TILE_BYTES), 0, 1024);
     const uint64_t vd = make_smem_desc(smem_u32(sV + st * C::TILE_BYTES), 16384, 1024);
     float s[64];
@@ -121,14 +137,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
     }
     wgmma_commit();
     wgmma_wait<0>();
-    // masking only on the diagonal / ragged last tile
+    // masking only on the diagonal / ragged last tile (DOC: and on tiles that start before some row's document)
     const int kv0 = j * 128;
-    if (j == qt || kv0 + 128 > S) {
+    if (j == qt || kv0 + 128 > S || (DOC && kv0 < tile_doc_hi)) {
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int kv = kv0 + 8 * (i >> 2) + cq + (i & 1);
         const int q = r_lo + 8 * ((i >> 1) & 1);
-        if (kv > q || kv >= S) s[i] = -INFINITY;
+        if (kv > q || kv >= S || (DOC && kv < doc_lo[(i >> 1) & 1])) s[i] = -INFINITY;
       }
     }
     float corr[2];
@@ -138,7 +154,10 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * hh], s[4 * jj + 2 * hh + 1]));
       const float m_new = fmaxf(m_run[hh], quad_max(mx) * scale_log2);
-      corr[hh] = exp2f(m_run[hh] - m_new);
+      // DOC: a row whose document starts after this tile has seen no key yet (m_new = -inf); subtracting 0 instead
+      // keeps exp2(-inf - m) at 0 rather than NaN.  Plain causal rows always see key 0 in the first tile.
+      const float m_sub = (DOC && m_new == -INFINITY) ? 0.f : m_new;
+      corr[hh] = exp2f(m_run[hh] - m_sub);
       m_run[hh] = m_new;
       float ls = 0.f;
 #pragma unroll
@@ -146,7 +165,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tm, __nv_bfloat16* __restric
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int i = 4 * jj + 2 * hh + e;
-          s[i] = exp2f(fmaf(s[i], scale_log2, -m_new));
+          s[i] = exp2f(fmaf(s[i], scale_log2, -m_sub));
           ls += s[i];
         }
       }
@@ -231,11 +250,13 @@ struct BwdCfg {
 //            acc1 (dV) += P^T Y2, acc2 (dK) += dS^T Y1.
 // MODE_DQ:   X1 = Q, X2 = dO (128 q rows), streamed Y1 = K, Y2 = V (64 kv rows);  S = X1 Y1^T, dP = X2 Y2^T,
 //            acc2 (dQ) += dS Y1.
-template <int HD, int MODE>
+// DOC: seg_plane = seg1 (document ends) for MODE_DKDV, seg0 (document starts) for MODE_DQ.
+template <int HD, int MODE, bool DOC>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constant__ CUtensorMap tm_do,
                 const float* __restrict__ lse2g, const float* __restrict__ delta, __nv_bfloat16* __restrict__ dqkv,
-                int S, int H, int KVH, float scale, int n_t128, int ld, const float* __restrict__ rope) {
+                int S, int H, int KVH, float scale, int n_t128, int ld, const float* __restrict__ rope,
+                const int* __restrict__ seg_plane) {
   using C = BwdCfg<HD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -257,9 +278,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
   } else {
     t128 = n_t128 - 1 - blockIdx.x; head_lo = blockIdx.y; head_n = 1; kvh = blockIdx.y / G;
   }
-  // streamed 64-row tiles: dK/dV -> q tiles from the diagonal to the end; dQ -> kv tiles up to the diagonal
-  const int s_lo = (MODE == MODE_DKDV) ? 2 * t128 : 0;
-  const int s_hi = (MODE == MODE_DKDV) ? n_t64 : min(2 * t128 + 2, n_t64);
+  // DOC: the document bound of the tile's first and last resident row (dK/dV: end, dQ: start)
+  const int* srow = DOC ? seg_plane + static_cast<size_t>(b) * S : nullptr;
+  const int tile_doc_first = DOC ? srow[t128 * 128] : 0;
+  const int tile_doc_last = DOC ? srow[min(t128 * 128 + 127, S - 1)] : 0;
+  // streamed 64-row tiles: dK/dV -> q tiles from the diagonal to the end (DOC: to the last document end of the tile);
+  // dQ -> kv tiles up to the diagonal (DOC: from the first document start of the tile)
+  const int s_lo = (MODE == MODE_DKDV) ? 2 * t128 : (DOC ? tile_doc_first / 64 : 0);
+  const int s_hi = (MODE == MODE_DKDV) ? (DOC ? tile_doc_last / 64 + 1 : n_t64) : min(2 * t128 + 2, n_t64);
   const int per_head = s_hi - s_lo;
   const int n_iter = per_head * head_n;
   const int xrow0 = b * S + t128 * 128;
@@ -317,6 +343,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
 #pragma unroll
   for (int i = 0; i < (MODE == MODE_DKDV ? HD / 2 : 1); ++i) acc1[i] = 0.f;
   float row_nl[2] = {0.f, 0.f}, row_nd[2] = {0.f, 0.f};
+  int row_doc[2] = {0, 0};                   // DOC: document bound of the thread's resident rows
+  if constexpr (DOC) {
+    row_doc[0] = srow[min(x_lo, S - 1)];
+    row_doc[1] = srow[min(x_lo + 8, S - 1)];
+  }
   if constexpr (MODE == MODE_DQ) {
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
@@ -362,7 +393,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
     // P and dS (unscaled) in place of S and dP
     // only tiles that touch the causal diagonal or cross the sequence end need per-element masking
     const bool diag = (MODE == MODE_DKDV) ? (y0 < t128 * 128 + 128) : (y0 + 64 > t128 * 128);
-    const bool need_mask = diag || (y0 + 64 > S) || (t128 * 128 + 128 > S);
+    // DOC: also tiles that reach past the first row's document end (dK/dV) or start before the last row's document (dQ)
+    const bool doc_edge = DOC && ((MODE == MODE_DKDV) ? (y0 + 63 > tile_doc_first) : (y0 < tile_doc_last));
+    const bool need_mask = diag || (y0 + 64 > S) || (t128 * 128 + 128 > S) || doc_edge;
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
       const int x = x_lo + 8 * ((i >> 1) & 1);
@@ -372,6 +405,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
       else { nl = row_nl[(i >> 1) & 1]; nd = row_nd[(i >> 1) & 1]; }
       bool masked = false;
       if (need_mask) masked = (MODE == MODE_DKDV) ? (x > y || y >= S || x >= S) : (y > x || y >= S || x >= S);
+      if constexpr (DOC) {
+        const int bound = row_doc[(i >> 1) & 1];
+        if (need_mask) masked = masked || ((MODE == MODE_DKDV) ? (y > bound) : (y < bound));
+      }
       const float pv = masked ? 0.f : exp2f(fmaf(s[i], scale_log2, nl));
       s[i] = pv;
       dp[i] = masked ? 0.f : pv * (dp[i] + nd);
@@ -425,13 +462,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tm_qkv, const __grid_constan
   }
 }
 
-template <int HD>
-static int launch_fwd(const void* qkv, void* o, float* lse, int B, int S, int H, int KVH, float scale, cudaStream_t st) {
+template <int HD, bool DOC>
+static int launch_fwd(const void* qkv, void* o, float* lse, int B, int S, int H, int KVH, float scale, const int* seg,
+                      cudaStream_t st) {
   using C = FwdCfg<HD>;
   CUtensorMap tm;
   const int W = (H + 2 * KVH) * HD;
   if (make_tmap_2d_bf16(&tm, qkv, (uint64_t)W, (uint64_t)B * S, (uint64_t)W, 64, 128)) return -3;
-  auto kern = attn_fwd_kernel<HD>;
+  auto kern = attn_fwd_kernel<HD, DOC>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
@@ -439,13 +477,14 @@ static int launch_fwd(const void* qkv, void* o, float* lse, int B, int S, int H,
     configured = true;
   }
   const int n_qt = (S + 127) / 128;
-  kern<<<dim3(n_qt, H, B), ATT_THREADS, C::SMEM, st>>>(tm, (__nv_bfloat16*)o, lse, S, H, KVH, scale * LOG2E, n_qt);
+  kern<<<dim3(n_qt, H, B), ATT_THREADS, C::SMEM, st>>>(tm, (__nv_bfloat16*)o, lse, S, H, KVH, scale * LOG2E, n_qt,
+                                                       seg);
   return (int)cudaGetLastError();
 }
 
-template <int HD>
+template <int HD, bool DOC>
 static int launch_bwd(const void* dout, const void* qkv, const void* o, const float* lse, void* dqkv, float* delta,
-                      int B, int S, int H, int KVH, float scale, const float* rope, cudaStream_t st) {
+                      int B, int S, int H, int KVH, float scale, const float* rope, const int* seg, cudaStream_t st) {
   using C = BwdCfg<HD>;
   const int W = (H + 2 * KVH) * HD;
   CUtensorMap q64, d64;
@@ -460,8 +499,8 @@ static int launch_bwd(const void* dout, const void* qkv, const void* o, const fl
     attn_delta_kernel<HD><<<(unsigned)blocks, 256, 0, st>>>((const __nv_bfloat16*)dout, (const __nv_bfloat16*)o, delta,
                                                             lse, lse2, B, S, H, ld);
   }
-  auto j1 = attn_bwd_kernel<HD, MODE_DKDV>;
-  auto j2 = attn_bwd_kernel<HD, MODE_DQ>;
+  auto j1 = attn_bwd_kernel<HD, MODE_DKDV, DOC>;
+  auto j2 = attn_bwd_kernel<HD, MODE_DQ, DOC>;
   static bool configured = false;
   if (!configured) {
     cudaError_t e = cudaFuncSetAttribute(j1, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
@@ -471,28 +510,41 @@ static int launch_bwd(const void* dout, const void* qkv, const void* o, const fl
     configured = true;
   }
   const int n_t = (S + 127) / 128;
+  const int* seg1 = DOC ? seg + (size_t)B * S : nullptr;   // dK/dV bounds its q range by document ends, dQ by starts
   j1<<<dim3(n_t, KVH, B), ATT_THREADS, C::SMEM, st>>>(q64, d64, lse2, delta, (__nv_bfloat16*)dqkv, S, H, KVH, scale, n_t,
-                                                      ld, rope);
+                                                      ld, rope, seg1);
   j2<<<dim3(n_t, H, B), ATT_THREADS, C::SMEM, st>>>(q64, d64, lse2, delta, (__nv_bfloat16*)dqkv, S, H, KVH, scale, n_t,
-                                                    ld, rope);
+                                                    ld, rope, seg);
   return (int)cudaGetLastError();
 }
 
 }  // namespace b200
 
+// seg (optional): [2][B*S] int32 document table (first | last position of each position's document within its row);
+// nullptr = plain causal attention
 extern "C" int b200_attn_fwd(const void* qkv, void* o, float* lse, int B, int S, int H, int KVH, int HD, float scale,
-                             cudaStream_t st) {
+                             cudaStream_t st, const int* seg) {
   if (H % KVH) return -1;
-  if (HD == 128) return b200::launch_fwd<128>(qkv, o, lse, B, S, H, KVH, scale, st);
-  if (HD == 64) return b200::launch_fwd<64>(qkv, o, lse, B, S, H, KVH, scale, st);
+  if (seg) {
+    if (HD == 128) return b200::launch_fwd<128, true>(qkv, o, lse, B, S, H, KVH, scale, seg, st);
+    if (HD == 64) return b200::launch_fwd<64, true>(qkv, o, lse, B, S, H, KVH, scale, seg, st);
+    return -2;
+  }
+  if (HD == 128) return b200::launch_fwd<128, false>(qkv, o, lse, B, S, H, KVH, scale, nullptr, st);
+  if (HD == 64) return b200::launch_fwd<64, false>(qkv, o, lse, B, S, H, KVH, scale, nullptr, st);
   return -2;
 }
 // rope (optional): [S][HD/2][cos, sin] table; dq and dk leave the kernel with the inverse rotation applied
 extern "C" int b200_attn_bwd(const void* dout, const void* qkv, const void* o, const float* lse, void* dqkv,
                              float* delta, int B, int S, int H, int KVH, int HD, float scale, const float* rope,
-                             cudaStream_t st) {
+                             cudaStream_t st, const int* seg) {
   if (H % KVH) return -1;
-  if (HD == 128) return b200::launch_bwd<128>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, st);
-  if (HD == 64) return b200::launch_bwd<64>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, st);
+  if (seg) {
+    if (HD == 128) return b200::launch_bwd<128, true>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, seg, st);
+    if (HD == 64) return b200::launch_bwd<64, true>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, seg, st);
+    return -2;
+  }
+  if (HD == 128) return b200::launch_bwd<128, false>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, nullptr, st);
+  if (HD == 64) return b200::launch_bwd<64, false>(dout, qkv, o, lse, dqkv, delta, B, S, H, KVH, scale, rope, nullptr, st);
   return -2;
 }

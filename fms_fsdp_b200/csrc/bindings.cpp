@@ -58,9 +58,9 @@ DECL int b200_ce_grad_inplace(void*, const long long*, const float*, float*, int
 DECL int b200_adamw(float*, const void*, int, float*, float*, void*, long long, float, float, float, float, float,
                     float, float, const float*, cudaStream_t);
 DECL int b200_sumsq(const void*, int, long long, float*, cudaStream_t);
-DECL int b200_attn_fwd(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t);
+DECL int b200_attn_fwd(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t, const int*);
 DECL int b200_attn_bwd(const void*, const void*, const void*, const float*, void*, float*, int, int, int, int, int,
-                       float, const float*, cudaStream_t);
+                       float, const float*, cudaStream_t, const int*);
 DECL void b200_gemm2_set_rope(const float*, int, int, int);
 DECL void b200_gemm2_set_swiglu(void*, int, int, int);
 DECL int b200_gemm2_fp8(const void*, const void*, void*, const float*, const float*, int, int, int, int, int, int, cudaStream_t);
@@ -343,26 +343,38 @@ void sumsq(const at::Tensor& x, at::Tensor& out) {
         "sumsq");
 }
 
+// optional document table of a packed batch: [2, B*S] int32 (document start | end per position), nullptr = causal
+const int* seg_ptr(const c10::optional<at::Tensor>& seg, const at::Tensor& qkv, int64_t B, int64_t S) {
+  if (!seg.has_value() || !seg->defined()) return nullptr;
+  TORCH_CHECK(seg->scalar_type() == at::kInt, "seg has dtype ", seg->scalar_type(), ", expected int32");
+  TORCH_CHECK(seg->is_contiguous(), "seg must be contiguous");
+  TORCH_CHECK(seg->device() == qkv.device(), "seg must be on the device of qkv");
+  TORCH_CHECK(seg->numel() == 2 * B * S, "seg must be a [2, B*S] table");
+  return seg->data_ptr<int>();
+}
+
 std::vector<at::Tensor> attn_fwd(const at::Tensor& qkv, int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd,
-                                 double scale) {
+                                 double scale, const c10::optional<at::Tensor>& seg) {
   c10::cuda::CUDAGuard guard(qkv.device());
   need(qkv, "qkv", at::kBFloat16);
   TORCH_CHECK(qkv.is_contiguous());
+  const int* seg_p = seg_ptr(seg, qkv, B, S);
   auto o = at::empty({B * S, H * hd}, qkv.options());
   auto lse = at::empty({B, H, S}, qkv.options().dtype(at::kFloat));
   check(b200_attn_fwd(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, S, H, KVH, hd, (float)scale,
-                      cur_stream()), "attn_fwd");
+                      cur_stream(), seg_p), "attn_fwd");
   return {o, lse};
 }
 at::Tensor attn_bwd(const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o, const at::Tensor& lse,
                     int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd, double scale,
-                    const c10::optional<at::Tensor>& rope) {
+                    const c10::optional<at::Tensor>& rope, const c10::optional<at::Tensor>& seg) {
   c10::cuda::CUDAGuard guard(qkv.device());
   need(qkv, "qkv", at::kBFloat16);
   need(dout, "do", at::kBFloat16);
   need(o, "o", at::kBFloat16);
   need(lse, "lse", at::kFloat);
   TORCH_CHECK(qkv.is_contiguous() && dout.is_contiguous() && o.is_contiguous() && lse.is_contiguous());
+  const int* seg_p = seg_ptr(seg, qkv, B, S);
   auto dqkv = at::empty_like(qkv);
   // [2 planes: delta | lse*log2e][B][H][S padded to 128]
   auto delta = at::empty({2, B, H, ((S + 127) / 128) * 128}, qkv.options().dtype(at::kFloat));
@@ -373,7 +385,8 @@ at::Tensor attn_bwd(const at::Tensor& dout, const at::Tensor& qkv, const at::Ten
     rope_p = rope->data_ptr<float>();
   }
   check(b200_attn_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
-                      delta.data_ptr<float>(), B, S, H, KVH, hd, (float)scale, rope_p, cur_stream()), "attn_bwd", 3);
+                      delta.data_ptr<float>(), B, S, H, KVH, hd, (float)scale, rope_p, cur_stream(), seg_p),
+        "attn_bwd", 3);
   return dqkv;
 }
 
@@ -767,9 +780,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("ce_grad_inplace", &ce_grad_inplace);
   m.def("adamw", &adamw);
   m.def("sumsq", &sumsq);
-  m.def("attn_fwd", &attn_fwd);
+  m.def("attn_fwd", &attn_fwd, py::arg("qkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("KVH"), py::arg("hd"),
+        py::arg("scale"), py::arg("seg") = py::none());
   m.def("attn_bwd", &attn_bwd, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("B"), py::arg("S"),
-        py::arg("H"), py::arg("KVH"), py::arg("hd"), py::arg("scale"), py::arg("rope") = py::none());
+        py::arg("H"), py::arg("KVH"), py::arg("hd"), py::arg("scale"), py::arg("rope") = py::none(),
+        py::arg("seg") = py::none());
   m.def("p2p_allgather", &p2p_allgather);
   m.def("reduce_scatter", &reduce_scatter, py::arg("peer_ptrs"), py::arg("out32"), py::arg("elem_offset"), py::arg("world"),
         py::arg("rank"), py::arg("src_bf16"), py::arg("scale"), py::arg("sumsq_out"), py::arg("max_ctas") = 0);

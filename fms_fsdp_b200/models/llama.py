@@ -47,6 +47,10 @@ class LLaMAConfig:
     # extension (not an fms field): HF-style frequency rescaling of long-context checkpoints, e.g. Llama 3.1
     # {"rope_type": "llama3", "factor": 8.0, "low_freq_factor": 1.0, "high_freq_factor": 4.0, "original_max_position_embeddings": 8192}
     rope_scaling: Optional[dict] = None
+    # extension (not an fms field): token id that ends a document in packed rows (the loader's eos_token).  When set,
+    # attention is masked at document boundaries.  RoPE positions stay absolute: rotary scores depend only on position
+    # differences, so a document in the middle of a row attends exactly as it would from position 0.
+    doc_separator: Optional[int] = None
 
     @property
     def hidden_dim(self) -> int:
@@ -196,18 +200,21 @@ class LLaMABlock(nn.Module):
         self.ff_sub_layer = GatedLinearUnit(cfg, device, dtype)
         object.__setattr__(self, "_rot", rot_emb)  # shared, not a submodule (no params, not in state dict)
 
-    def forward(self, x):
+    def forward(self, x, doc=None):
+        """``doc``: the ``ops.document_segments`` table of a packed batch; given one, the block returns ``(x, doc)``
+        so the table travels with the hidden state from block to block."""
         a, cfg = self.attn, self.config
         B, S, _ = x.shape
         h, x = self.ln.fork(x)
         # projection + RoPE + attention: one node, RoPE fused into the GEMM / dq-dk epilogues
         ctx = ops.qkv_attention(h, a.in_proj.qkv_fused.weight, self._rot.table(x.device, S), a.nheads, a.kvheads,
-                                a.head_dim)
+                                a.head_dim, doc=doc)
         x = a.dense(ctx, residual=x)
         h, x = self.ff_ln.fork(x)
         ff = self.ff_sub_layer
         # gate/up GEMM with the SwiGLU epilogue, down projection with the residual epilogue: one autograd node
-        return ops.gated_mlp(h, ff.wg1_fused.weight, ff.w2.weight, residual=x)
+        x = ops.gated_mlp(h, ff.wg1_fused.weight, ff.w2.weight, residual=x)
+        return x if doc is None else (x, doc)
 
 
 class LLaMA(nn.Module):
@@ -241,8 +248,14 @@ class LLaMA(nn.Module):
     # ---- plain (unsharded) forward: logits, as the reference model returns
     def forward(self, x, labels=None, return_hidden: bool = False):
         h = self.shared(x)
-        for blk in self.layers:
-            h = blk(h)
+        if self.config.doc_separator is None:
+            for blk in self.layers:
+                h = blk(h)
+        else:
+            state = (h, ops.document_segments(x, self.config.doc_separator))
+            for blk in self.layers:
+                state = blk(*state)
+            h = state[0]
         h = self.dec_norm(h)
         if return_hidden:
             return h
@@ -257,9 +270,19 @@ class LLaMA(nn.Module):
         return list(self.layers), [self.shared, self.dec_norm]
 
     def engine_embed(self, tokens):
-        return self.shared(tokens)
+        h = self.shared(tokens)
+        if self.config.doc_separator is None:
+            return h
+        return h, ops.document_segments(tokens, self.config.doc_separator)
 
-    def engine_head(self, h, labels=None, ignore_index=-100):
+    def engine_head(self, h, *args, **kwargs):
+        """``engine_head(h, labels=None, ignore_index=-100)``; with ``doc_separator`` set the engine's state is
+        ``(h, seg)`` and the document table that follows ``h`` is ignored here."""
+        if self.config.doc_separator is not None:
+            args = args[1:]
+        return self._head(h, *args, **kwargs)
+
+    def _head(self, h, labels=None, ignore_index=-100):
         h = self.dec_norm(h)
         if labels is None:
             return self.shared(h, reverse=True)

@@ -354,37 +354,44 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, inverse=
 
 
 # ------------------------------------------------------------------------------------- attention
-def _sdpa_fwd(qkv, B, S, H, KVH, hd, scale):
+def _sdpa_fwd(qkv, B, S, H, KVH, hd, scale, seg=None):
     q, k, v = torch_kernels._split_qkv(qkv, B, S, H, KVH, hd)
     q, k, v = (t.transpose(1, 2) for t in (q, k, v))
-    o = torch.nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True, scale=scale, enable_gqa=(KVH != H))
+    if seg is not None:
+        mask = torch_kernels.document_mask(seg, B, S).unsqueeze(1)
+        o = torch.nn.functional.scaled_dot_product_attention(q, k, v, attn_mask=mask, scale=scale,
+                                                             enable_gqa=(KVH != H))
+    else:
+        o = torch.nn.functional.scaled_dot_product_attention(q, k, v, is_causal=True, scale=scale,
+                                                             enable_gqa=(KVH != H))
     return o.transpose(1, 2).reshape(B * S, H * hd).contiguous()
 
 
-def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
+def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True, seg=None):
+    """``seg``: [2, B*S] int32 document table of a packed batch (``ops.document_segments``); None = causal."""
     if ATTN_IMPL == "wgmma" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
-        o, lse = _C.attn_fwd(qkv.contiguous(), B, S, H, KVH, hd, float(scale))
+        o, lse = _C.attn_fwd(qkv.contiguous(), B, S, H, KVH, hd, float(scale), seg)
         return o, lse
     if ATTN_IMPL == "sdpa":
-        return _sdpa_fwd(qkv, B, S, H, KVH, hd, scale), torch.empty(0, device=qkv.device)
-    return _fallback("attn_fwd").attn_fwd(qkv, B, S, H, KVH, hd, scale, causal)
+        return _sdpa_fwd(qkv, B, S, H, KVH, hd, scale, seg), torch.empty(0, device=qkv.device)
+    return _fallback("attn_fwd").attn_fwd(qkv, B, S, H, KVH, hd, scale, causal, seg=seg)
 
 
-def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=None):
+def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=None, seg=None):
     """``rope_table``: the forward applied RoPE (full head_dim, interleaved) to q, k before this attention; return the
     gradient of the UN-rotated projection (inverse rotation fused into the dq / dk epilogues)."""
     if ATTN_IMPL == "wgmma" and qkv.dtype == torch.bfloat16 and hd in (64, 128) and causal:
-        return _C.attn_bwd(do.contiguous(), qkv.contiguous(), o, lse, B, S, H, KVH, hd, float(scale), rope_table)
+        return _C.attn_bwd(do.contiguous(), qkv.contiguous(), o, lse, B, S, H, KVH, hd, float(scale), rope_table, seg)
     if rope_table is not None:
-        g = attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal)
+        g = attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal, seg=seg)
         return rope_(g, rope_table, S, H, KVH, hd, inverse=True)
     if ATTN_IMPL == "sdpa":
         with torch.enable_grad():
             leaf = qkv.detach().requires_grad_(True)
-            out = _sdpa_fwd(leaf, B, S, H, KVH, hd, scale)
+            out = _sdpa_fwd(leaf, B, S, H, KVH, hd, scale, seg)
             (g,) = torch.autograd.grad(out, leaf, do)
         return g
-    return _fallback("attn_bwd").attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal)
+    return _fallback("attn_bwd").attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal, seg=seg)
 
 
 # ---------------------------------------------------------------------------------------- SwiGLU

@@ -269,13 +269,29 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, interlea
 
 
 # --------------------------------------------------------------------------------------- attention
+def document_segments(tokens, sep: int):
+    """Document table of a packed batch ``tokens`` [B, S]: int32 [2, B*S], row 0 the first and row 1 the last position
+    (within its row) of the document that holds each position.  A ``sep`` token ends its document; position 0 of every
+    row starts one.  Device-side scans only (no host synchronisation)."""
+    B, S = tokens.shape
+    pos = torch.arange(S, device=tokens.device).expand(B, S)
+    is_sep = tokens == sep
+    # start: one past the last separator strictly before s
+    after = torch.where(is_sep, pos + 1, torch.zeros_like(pos)).cummax(dim=1).values
+    start = torch.cat([torch.zeros_like(after[:, :1]), after[:, :-1]], dim=1)
+    # end: the first separator at or after s, else the row's last position
+    at = torch.where(is_sep, pos, torch.full_like(pos, S - 1))
+    end = at.flip(1).cummin(dim=1).values.flip(1)
+    return torch.stack([start.reshape(-1), end.reshape(-1)]).to(torch.int32).contiguous()
+
+
 class _Attention(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, qkv, B, S, H, KVH, hd, scale):
+    def forward(ctx, qkv, B, S, H, KVH, hd, scale, seg):
         K = kernels_for(qkv)
         q2 = qkv.view(B * S, -1)
-        o, lse = K.attn_fwd(q2, B, S, H, KVH, hd, scale)
-        ctx.K, ctx.args = K, (B, S, H, KVH, hd, scale)
+        o, lse = K.attn_fwd(q2, B, S, H, KVH, hd, scale, seg=seg)
+        ctx.K, ctx.args, ctx.seg = K, (B, S, H, KVH, hd, scale), seg
         ctx.save_for_backward(qkv, o, lse)
         return o.view(B, S, H * hd)
 
@@ -284,8 +300,8 @@ class _Attention(torch.autograd.Function):
         qkv, o, lse = ctx.saved_tensors
         B, S, H, KVH, hd, scale = ctx.args
         dqkv = ctx.K.attn_bwd(do.reshape(B * S, H * hd).contiguous(), qkv.view(B * S, -1), o, lse,
-                              B, S, H, KVH, hd, scale)
-        return dqkv.view_as(qkv), None, None, None, None, None, None
+                              B, S, H, KVH, hd, scale, seg=ctx.seg)
+        return dqkv.view_as(qkv), None, None, None, None, None, None, None
 
 
 class _QKVAttention(torch.autograd.Function):
@@ -294,13 +310,13 @@ class _QKVAttention(torch.autograd.Function):
     (SURVEY.md K1-K3; reference path: fms MultiHeadAttention.in_proj -> RotaryEmbedding.adjusted_qk -> SDPA)."""
 
     @staticmethod
-    def forward(ctx, h, w, table, S, H, KVH, hd, scale):
+    def forward(ctx, h, w, table, S, H, KVH, hd, scale, seg):
         K = kernels_for(h)
         B = h.shape[0]
         h2 = h.reshape(-1, h.shape[-1])
         qkv = K.gemm(h2, _wdata(w), "nt", rope=(table, S, hd, H, KVH))
-        o, lse = K.attn_fwd(qkv, B, S, H, KVH, hd, scale)
-        ctx.K, ctx.w, ctx.args = K, w, (B, S, H, KVH, hd, scale)
+        o, lse = K.attn_fwd(qkv, B, S, H, KVH, hd, scale, seg=seg)
+        ctx.K, ctx.w, ctx.args, ctx.seg = K, w, (B, S, H, KVH, hd, scale), seg
         ctx.save_for_backward(h, qkv, o, lse, table)
         return o.view(B, S, H * hd)
 
@@ -310,29 +326,32 @@ class _QKVAttention(torch.autograd.Function):
         B, S, H, KVH, hd, scale = ctx.args
         K, w = ctx.K, ctx.w
         dqkv = K.attn_bwd(do.reshape(B * S, H * hd).contiguous(), qkv, o, lse, B, S, H, KVH, hd, scale,
-                          rope_table=table)
+                          rope_table=table, seg=ctx.seg)
         h2 = h.reshape(-1, h.shape[-1])
         dh = K.gemm(dqkv, _wdata(w), "nn").view_as(h) if ctx.needs_input_grad[0] else None
         dw = None
         if ctx.needs_input_grad[1]:
             dw = _deliver_wgrad(w, lambda out, acc: K.gemm(dqkv, h2, "tn", out=out, accumulate=acc))
-        return dh, dw, None, None, None, None, None, None
+        return dh, dw, None, None, None, None, None, None, None
 
 
-def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None):
-    """attention(rope(h @ w^T)) for a fused [(H + 2 KVH) * hd, D] projection weight; h: [B, S, D]."""
+def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None):
+    """attention(rope(h @ w^T)) for a fused [(H + 2 KVH) * hd, D] projection weight; h: [B, S, D].  ``doc``: the
+    ``document_segments`` table of a packed batch (attention stays inside each document), None = causal."""
     S = h.shape[1]
     scale = (head_dim ** -0.5) if scale is None else scale
     if _GEMM_PRECISION == "fp8":     # fp8 projection, then the stand-alone RoPE kernel and attention
-        return attention(rope_(linear(h, w), table, S, nheads, kvheads, head_dim), nheads, kvheads, head_dim, scale)
-    return _QKVAttention.apply(h, w, table, S, nheads, kvheads, head_dim, scale)
+        return attention(rope_(linear(h, w), table, S, nheads, kvheads, head_dim), nheads, kvheads, head_dim, scale,
+                         doc=doc)
+    return _QKVAttention.apply(h, w, table, S, nheads, kvheads, head_dim, scale, doc)
 
 
-def attention(qkv, nheads, kvheads, head_dim, scale=None):
-    """Causal GQA flash attention on a fused (roped) projection [B, S, (H+2KVH)*hd] -> [B, S, H*hd]."""
+def attention(qkv, nheads, kvheads, head_dim, scale=None, doc=None):
+    """Causal GQA flash attention on a fused (roped) projection [B, S, (H+2KVH)*hd] -> [B, S, H*hd].  ``doc``: the
+    ``document_segments`` table of a packed batch (a query sees only keys of its own document), None = causal."""
     B, S, _ = qkv.shape
     scale = (head_dim ** -0.5) if scale is None else scale
-    return _Attention.apply(qkv, B, S, nheads, kvheads, head_dim, scale)
+    return _Attention.apply(qkv, B, S, nheads, kvheads, head_dim, scale, doc)
 
 
 # ------------------------------------------------------------------------------------------ swiglu

@@ -164,7 +164,14 @@ def _split_qkv(qkv, B, S, H, KVH, hd):
     return t[:, :, :H], t[:, :, H:H + KVH], t[:, :, H + KVH:]
 
 
-def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
+def document_mask(seg, B, S):
+    """[B, S, S] bool visibility of a packed batch: key k is visible to query q when seg[0][q] <= k <= q."""
+    start = seg[0].view(B, S).long()
+    k = torch.arange(S, device=seg.device)
+    return (k.view(1, 1, S) >= start.unsqueeze(-1)) & (k.view(1, 1, S) <= k.view(1, S, 1))
+
+
+def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True, seg=None):
     q, k, v = _split_qkv(qkv, B, S, H, KVH, hd)
     qf, kf, vf = (t.permute(0, 2, 1, 3).float() for t in (q, k, v))
     rep = H // KVH
@@ -172,7 +179,9 @@ def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
         kf = kf.repeat_interleave(rep, dim=1)
         vf = vf.repeat_interleave(rep, dim=1)
     s = (qf @ kf.transpose(-1, -2)) * scale
-    if causal:
+    if seg is not None:
+        s = s.masked_fill(~document_mask(seg, B, S).unsqueeze(1), float("-inf"))
+    elif causal:
         mask = torch.ones(S, S, dtype=torch.bool, device=qkv.device).tril()
         s = s.masked_fill(~mask, float("-inf"))
     lse = torch.logsumexp(s, dim=-1)
@@ -181,9 +190,9 @@ def attn_fwd(qkv, B, S, H, KVH, hd, scale, causal=True):
     return o, lse
 
 
-def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=None):
+def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=None, seg=None):
     if rope_table is not None:   # gradient of the un-rotated projection
-        g = attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal)
+        g = attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal, seg=seg)
         return rope_(g, rope_table, S, H, KVH, hd, inverse=True)
     q, k, v = _split_qkv(qkv, B, S, H, KVH, hd)
     qf, kf, vf = (t.permute(0, 2, 1, 3).float() for t in (q, k, v))
@@ -193,7 +202,9 @@ def attn_bwd(do, qkv, o, lse, B, S, H, KVH, hd, scale, causal=True, rope_table=N
     dof = do.view(B, S, H, hd).permute(0, 2, 1, 3).float()
     of = o.view(B, S, H, hd).permute(0, 2, 1, 3).float()
     s = (qf @ kx.transpose(-1, -2)) * scale
-    if causal:
+    if seg is not None:
+        s = s.masked_fill(~document_mask(seg, B, S).unsqueeze(1), float("-inf"))
+    elif causal:
         mask = torch.ones(S, S, dtype=torch.bool, device=qkv.device).tril()
         s = s.masked_fill(~mask, float("-inf"))
     p = torch.exp(s - lse.unsqueeze(-1))

@@ -54,6 +54,9 @@ def main(**kwargs):
      param_init_fn) = get_policies(cfg, rank, block)
 
     llama_config = get_model_config(cfg.model_variant)
+    if cfg.document_attention_mask:
+        # packed lines hold several documents, each ended by the loader's eos_token: attend within a document only
+        llama_config.doc_separator = cfg.eos_token
     if cfg.low_cpu_fsdp or use_cuda:
         # one unit at a time is materialised directly on the device by the sharded runtime
         with torch.device("meta"):

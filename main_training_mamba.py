@@ -25,6 +25,10 @@ from fms_fsdp_b200.utils.train_utils import (get_policies, get_profiler, lr_sche
 def main(**kwargs):
     cfg = config.train_config()
     update_config(cfg, **kwargs)
+    if cfg.document_attention_mask:
+        raise ValueError("--document_attention_mask is not supported for Mamba models: the SSD scan and the causal "
+                         "conv1d carry state across document boundaries, so masking only the attention layers "
+                         "would not isolate documents")
 
     use_cuda = torch.cuda.is_available() and cfg.comm_backend != "gloo"
     if use_cuda:
