@@ -68,7 +68,7 @@ DECL int b200_quant_rowwise_e4m3(const void*, void*, float*, int, int, int, int,
 DECL void b200_gemm2_set_push(void* const*, long long, long long, int, int, int);
 DECL int b200_p2p_push_range(const void*, void* const*, long long, long long, long long, int, cudaStream_t);
 DECL int b200_p2p_allgather(const void* const*, void*, long long, int, int, cudaStream_t);
-DECL int b200_reduce_scatter(const void* const*, float*, long long, long long, int, int, int, float, float*,
+DECL int b200_reduce_scatter(const void* const*, float*, long long, long long, int, int, int, float, float*, int,
                              cudaStream_t);
 DECL int b200_allreduce_inplace(void* const*, long long, int, int, int, float, float*, cudaStream_t);
 DECL int b200_signal_barrier(uint32_t* const*, int, int, uint32_t, int, int, cudaStream_t);
@@ -397,13 +397,15 @@ void p2p_allgather(const at::Tensor& peer_ptrs, at::Tensor& full, int64_t shard_
                            cur_stream()), "p2p_allgather");
 }
 void reduce_scatter(const at::Tensor& peer_ptrs, at::Tensor& out32, int64_t elem_offset, int64_t world, int64_t rank,
-                    bool src_bf16, double scale, const c10::optional<at::Tensor>& sumsq_out, int64_t max_ctas) {
+                    bool src_bf16, double scale, const c10::optional<at::Tensor>& sumsq_out, int64_t max_ctas,
+                    bool accumulate) {
   c10::cuda::CUDAGuard guard(out32.device());
   need(out32, "out", at::kFloat);
   b200_comm_set_reduce_ctas(max_ctas > 0 ? (int)max_ctas : g_reduce_ctas_default);
   check(b200_reduce_scatter((const void* const*)peer_ptrs.data_ptr(), out32.data_ptr<float>(), out32.numel(),
                             elem_offset, world, rank, src_bf16, (float)scale,
-                            sumsq_out.has_value() ? sumsq_out->data_ptr<float>() : nullptr, cur_stream()),
+                            sumsq_out.has_value() ? sumsq_out->data_ptr<float>() : nullptr, accumulate ? 1 : 0,
+                            cur_stream()),
         "reduce_scatter");
 }
 void allreduce_inplace(const at::Tensor& peer_ptrs, int64_t numel, int64_t world, int64_t rank, bool is_bf16,
@@ -787,7 +789,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("seg") = py::none());
   m.def("p2p_allgather", &p2p_allgather);
   m.def("reduce_scatter", &reduce_scatter, py::arg("peer_ptrs"), py::arg("out32"), py::arg("elem_offset"), py::arg("world"),
-        py::arg("rank"), py::arg("src_bf16"), py::arg("scale"), py::arg("sumsq_out"), py::arg("max_ctas") = 0);
+        py::arg("rank"), py::arg("src_bf16"), py::arg("scale"), py::arg("sumsq_out"), py::arg("max_ctas") = 0,
+        py::arg("accumulate") = false);
   m.def("allreduce_inplace", &allreduce_inplace);
   m.def("signal_barrier", &signal_barrier, py::arg("pad_ptrs"), py::arg("world"), py::arg("rank"), py::arg("epoch"),
         py::arg("anchor"), py::arg("slot_base") = 0, py::arg("mode") = 0);

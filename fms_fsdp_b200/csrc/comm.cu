@@ -8,7 +8,8 @@
 //
 //   signal_barrier     all ranks of the group have reached this point of their stream
 //   p2p_allgather      full[r*n:(r+1)*n] = shard of rank r          (pull; parameter path, N7)
-//   reduce_scatter     out32 = scale * sum_r full_r[my slice] (+ sum of squares)   (gradient path, N8 + K11)
+//   reduce_scatter     out32 = scale * sum_r full_r[my slice] (+ sum of squares)   (gradient path, N8 + K11);
+//                      accumulate mode: out32 += scale * sum_r ... (gradient accumulation over micro-steps)
 //   allreduce_inplace  phase 1 of a two-phase all-reduce: reduce my slice in place (N9/N10)
 #include "common.cuh"
 
@@ -165,7 +166,8 @@ B200_DEVINL float block_sum256(float v, float* sh) {
 }
 
 // out[i] = scale * sum_r src_r[off + i]   (src bf16 or fp32, out fp32) ; sumsq += sum out^2
-template <bool SRC_BF16, int W>
+// ACC: out[i] += scale * sum_r src_r[off + i] ; sumsq += sum of the squared RESULT (the accumulated gradient)
+template <bool SRC_BF16, int W, bool ACC = false>
 __global__ void __launch_bounds__(256) reduce_scatter_kernel(const void* const* srcs, float* out, size_t n, size_t off,
                                                              int rank, float scale, float* sumsq) {
   __shared__ float sh[32];
@@ -196,12 +198,22 @@ __global__ void __launch_bounds__(256) reduce_scatter_kernel(const void* const* 
         acc[2] += __uint_as_float(v[r].z); acc[3] += __uint_as_float(v[r].w);
       }
     }
+    float4* o = reinterpret_cast<float4*>(out + i * VEC);
+    float prev[VEC];
+    if constexpr (ACC) {
+      const float4 p0 = o[0];
+      prev[0] = p0.x; prev[1] = p0.y; prev[2] = p0.z; prev[3] = p0.w;
+      if constexpr (SRC_BF16) {
+        const float4 p1 = o[1];
+        prev[4] = p1.x; prev[5] = p1.y; prev[6] = p1.z; prev[7] = p1.w;
+      }
+    }
 #pragma unroll
     for (int k = 0; k < VEC; ++k) {
       acc[k] *= scale;
+      if constexpr (ACC) acc[k] += prev[k];
       ss += acc[k] * acc[k];
     }
-    float4* o = reinterpret_cast<float4*>(out + i * VEC);
     o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
     if constexpr (SRC_BF16) o[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
   }
@@ -212,7 +224,7 @@ __global__ void __launch_bounds__(256) reduce_scatter_kernel(const void* const* 
 }
 
 // Any group size (HSDP 2x3, 6-GPU jobs ...): peer table read per iteration instead of W unrolled base registers.
-template <bool SRC_BF16>
+template <bool SRC_BF16, bool ACC = false>
 __global__ void __launch_bounds__(256) reduce_scatter_dyn_kernel(const void* const* srcs, float* out, size_t n, size_t off,
                                                                  int world, int rank, float scale, float* sumsq) {
   __shared__ float sh[32];
@@ -235,12 +247,22 @@ __global__ void __launch_bounds__(256) reduce_scatter_dyn_kernel(const void* con
         acc[2] += __uint_as_float(v.z); acc[3] += __uint_as_float(v.w);
       }
     }
+    float4* o = reinterpret_cast<float4*>(out + i * VEC);
+    float prev[VEC];
+    if constexpr (ACC) {
+      const float4 p0 = o[0];
+      prev[0] = p0.x; prev[1] = p0.y; prev[2] = p0.z; prev[3] = p0.w;
+      if constexpr (SRC_BF16) {
+        const float4 p1 = o[1];
+        prev[4] = p1.x; prev[5] = p1.y; prev[6] = p1.z; prev[7] = p1.w;
+      }
+    }
 #pragma unroll
     for (int k = 0; k < VEC; ++k) {
       acc[k] *= scale;
+      if constexpr (ACC) acc[k] += prev[k];
       ss += acc[k] * acc[k];
     }
-    float4* o = reinterpret_cast<float4*>(out + i * VEC);
     o[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
     if constexpr (SRC_BF16) o[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
   }
@@ -421,23 +443,33 @@ static int g_reduce_max_ctas = 132 * 2;
 extern "C" void b200_comm_set_reduce_ctas(int n) { g_reduce_max_ctas = n < 1 ? 1 : n; }
 
 #define RS_CASE(BF, WW) \
-  case WW: reduce_scatter_kernel<BF, WW><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, rank, scale, sumsq); break;
+  case WW: reduce_scatter_kernel<BF, WW, ACC><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, rank, scale, sumsq); break;
 
+template <bool ACC>
+static void launch_reduce_scatter(const void* const* srcs, float* out, long long n, long long off, int world, int rank,
+                                  int src_bf16, float scale, float* sumsq, int grid, cudaStream_t s) {
+  if (src_bf16) {
+    switch (world) { RS_CASE(true, 1) RS_CASE(true, 2) RS_CASE(true, 4) RS_CASE(true, 8)
+      default: reduce_scatter_dyn_kernel<true, ACC><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, world, rank, scale,
+                                                                        sumsq); }
+  } else {
+    switch (world) { RS_CASE(false, 1) RS_CASE(false, 2) RS_CASE(false, 4) RS_CASE(false, 8)
+      default: reduce_scatter_dyn_kernel<false, ACC><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, world, rank, scale,
+                                                                         sumsq); }
+  }
+}
+
+// accumulate != 0: out += scale * sum (micro-steps 2..k of gradient accumulation)
 extern "C" int b200_reduce_scatter(const void* const* srcs, float* out, long long n, long long off, int world, int rank,
-                                   int src_bf16, float scale, float* sumsq, cudaStream_t s) {
+                                   int src_bf16, float scale, float* sumsq, int accumulate, cudaStream_t s) {
   const int vec = src_bf16 ? 8 : 4;
   if (n % vec || off % vec) return -1;
   long long nvec = n / vec;
   int grid = (int)((nvec + 255) / 256);
   if (grid > g_reduce_max_ctas) grid = g_reduce_max_ctas;
   if (grid < 1) grid = 1;
-  if (src_bf16) {
-    switch (world) { RS_CASE(true, 1) RS_CASE(true, 2) RS_CASE(true, 4) RS_CASE(true, 8)
-      default: reduce_scatter_dyn_kernel<true><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, world, rank, scale, sumsq); }
-  } else {
-    switch (world) { RS_CASE(false, 1) RS_CASE(false, 2) RS_CASE(false, 4) RS_CASE(false, 8)
-      default: reduce_scatter_dyn_kernel<false><<<grid, 256, 0, s>>>(srcs, out, (size_t)n, (size_t)off, world, rank, scale, sumsq); }
-  }
+  if (accumulate) launch_reduce_scatter<true>(srcs, out, n, off, world, rank, src_bf16, scale, sumsq, grid, s);
+  else launch_reduce_scatter<false>(srcs, out, n, off, world, rank, src_bf16, scale, sumsq, grid, s);
   return (int)cudaGetLastError();
 }
 

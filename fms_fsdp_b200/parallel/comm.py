@@ -9,7 +9,9 @@ Interface (all ops are enqueued on the *current* stream of ``device``):
   alloc_shard / alloc_full     buffers the collectives may need to register (symmetric heap)
   all_gather(shard, full)      full[r*n:(r+1)*n] = shard of shard-rank r
   reduce_scatter(full, shard32, scale, sumsq)  shard32 = scale * sum_ranks(full)[my chunk]  (fp32),
-                               then replica all-reduce (HSDP), then sumsq += ||shard32||^2
+                               then replica all-reduce (HSDP), then sumsq += ||shard32||^2;
+                               ``accumulate=True``: shard32 += ... (gradient accumulation), ``replica=False``: the HSDP
+                               replica all-reduce is deferred to a later call (micro-steps before the last one)
   all_reduce_full(full, scale, sumsq)  NO_SHARD/DDP gradient path (in place on the full buffer)
 """
 from __future__ import annotations
@@ -66,14 +68,18 @@ class TorchCollectives:
         return t
 
     def reduce_scatter(self, full: torch.Tensor, shard32: torch.Tensor, scale: float,
-                       sumsq: Optional[torch.Tensor]):
+                       sumsq: Optional[torch.Tensor], accumulate: bool = False, replica: bool = True):
         m = self.mesh
         tmp = self._tmp(shard32.numel(), full.dtype)
         dist.reduce_scatter_tensor(tmp, full, op=dist.ReduceOp.SUM, group=m.shard_group)
-        shard32.copy_(tmp)
-        if m.replica_size > 1:
+        if accumulate:
+            shard32.add_(tmp.float(), alpha=scale)
+        else:
+            shard32.copy_(tmp)
+        if replica and m.replica_size > 1:
             dist.all_reduce(shard32, op=dist.ReduceOp.SUM, group=m.replica_group)
-        shard32.mul_(scale)
+        if not accumulate:
+            shard32.mul_(scale)
         if sumsq is not None:
             kernels_for(shard32).sumsq(shard32, out=sumsq)
 

@@ -77,10 +77,11 @@ class ShardUnit:
         for _, p in self.params:
             p.data = placeholder
 
-    def bind_grads(self, flat: torch.Tensor):
+    def bind_grads(self, flat: torch.Tensor, accumulate: bool = False):
+        """``accumulate``: the buffer already holds earlier micro-steps' gradients -- every producer adds to it."""
         for (_, p), s in zip(self.params, self.layout.slots):
             p._grad_buf = flat[s.offset:s.offset + s.numel].view(s.shape)
-            p._grad_ready = False
+            p._grad_ready = accumulate
             p.grad = None
 
     def bind_grads_push(self, vec: torch.Tensor, make_target):
@@ -129,8 +130,15 @@ class ShardedModel(nn.Module):
                  mixed_precision: Optional[MixedPrecision] = None, device: Optional[torch.device] = None,
                  collective_impl: str = "auto", prefetch_depth: int = 2, param_init_fn=None,
                  mesh: Optional[DPMesh] = None, local_world: Optional[int] = None,
-                 reshard_after_forward: bool = True, sync_module_states: bool = False, auto_wrap_policy=None):
-        """``sync_module_states``: broadcast global rank 0's initial parameters to every rank before sharding (torch
+                 reshard_after_forward: bool = True, sync_module_states: bool = False, auto_wrap_policy=None,
+                 grad_accum_steps: int = 1):
+        """``grad_accum_steps``: micro-steps (``forward_backward`` / ``forward_backward_custom`` / ``model(x)`` then
+        ``.backward()``) per optimizer step.  Their gradients are summed in fp32 and the optimizer sees the gradient of the
+        MEAN micro-batch loss: ``clip_grad_norm_`` reports ``sqrt(sum ||g||^2) / k`` and AdamW scales by ``clip / k``.
+        Sharded meshes reduce-scatter every micro-step into the fp32 shard (the HSDP replica all-reduce runs once, on the
+        last one); unsharded meshes (1 GPU, ddp) accumulate locally in an fp32 gradient buffer and communicate once.
+
+        ``sync_module_states``: broadcast global rank 0's initial parameters to every rank before sharding (torch
         FSDP's flag of the same name; the reference sets it for the speculator, ``train_speculator.py:205``).
 
         ``auto_wrap_policy``: predicate over the model's chain of blocks (``policies.get_wrapper(block_cls)``, the
@@ -138,6 +146,10 @@ class ShardedModel(nn.Module):
         just in time, released after use); a block for which it is false stays in the ROOT unit next to embedding / head
         / final norm -- resident for the whole step, reduced with the root.  ``None`` = every block is a unit."""
         super().__init__()
+        if int(grad_accum_steps) != grad_accum_steps or grad_accum_steps < 1:
+            raise ValueError(f"grad_accum_steps must be an integer >= 1, got {grad_accum_steps!r}")
+        self.grad_accum_steps = int(grad_accum_steps)
+        self._micro = 0                 # micro-steps run since the last optimizer step
         self.module = model
         self._sync_module_states = bool(sync_module_states)
         self.device = torch.device(device) if device is not None else (
@@ -227,6 +239,9 @@ class ShardedModel(nn.Module):
             self._warm_push_pool()
         self._gnorm_sq = torch.zeros((), dtype=torch.float32, device=self.device)
         self._clip_coef: Optional[torch.Tensor] = None
+        # AdamW's gradient multiplier when the step was not clipped (k > 1); persistent for the asynchronous optimizer
+        self._inv_accum = (torch.full((), 1.0 / self.grad_accum_steps, dtype=torch.float32, device=self.device)
+                           if self.grad_accum_steps > 1 else None)
         self._saved = None
         self.step_count = 0
         self.last_grad_norm: Optional[torch.Tensor] = None
@@ -328,12 +343,13 @@ class ShardedModel(nn.Module):
                 p.data = self._placeholder
             u.full = _Buf(u.lowp, self._event())
             u.bind_params(u.lowp)
+            # accumulating micro-steps in bf16 would round every partial sum: k > 1 keeps this buffer in fp32
+            gdt = self.mp.reduce_dtype if self.grad_accum_steps == 1 else torch.float32
             if self.mesh.replica_size == 1:
-                gdt = self.mp.reduce_dtype
                 u.grad_shard = torch.zeros(layout.total, dtype=gdt, device=self.device)
                 u.full_grad = _Buf(u.grad_shard, self._event())
             else:
-                u.grad_shard = self.coll.alloc_full(layout.total, self.mp.reduce_dtype)
+                u.grad_shard = self.coll.alloc_full(layout.total, gdt)
                 u.full_grad = _Buf(u.grad_shard, self._event())
         else:
             u.grad_shard = self.coll.alloc_grad_shard(n)
@@ -474,7 +490,8 @@ class ShardedModel(nn.Module):
         if self.is_cuda:
             self.s_compute.wait_event(u.full_grad.free_event)
         u.pushed = False
-        u.bind_grads(u.full_grad.t)
+        # unsharded gradient accumulation: micro-steps 2..k add into the persistent buffer
+        u.bind_grads(u.full_grad.t, accumulate=self.mesh.shard_size == 1 and self._micro > 1)
 
     def _push_eligible(self, u: ShardUnit) -> bool:
         """Block units whose every parameter is a norm-style vector or a weight matrix large enough for the fused-epilogue
@@ -526,6 +543,12 @@ class ShardedModel(nn.Module):
         u.unbind_grads()
         u._grads_bound = False
         m, W = self.mesh, self.mesh.world
+        # gradient accumulation: micro-step 1 overwrites the fp32 shard, later ones add; the HSDP replica all-reduce and
+        # ||g||^2 belong to the last micro-step only.  Unsharded meshes communicate once, after the last micro-step.
+        last = self._micro >= self.grad_accum_steps
+        if m.shard_size == 1 and not last:
+            return
+        acc = {} if self.grad_accum_steps == 1 else dict(accumulate=self._micro > 1, replica=last)
         ctx = torch.cuda.stream(self.s_reduce) if self.is_cuda else contextlib.nullcontext()
         if self.is_cuda:
             self.s_reduce.wait_stream(self.s_compute)
@@ -535,14 +558,14 @@ class ShardedModel(nn.Module):
             elif getattr(u, "pushed", False):
                 if u.layout.matrix_begin:
                     self.coll.push_vectors(u.vec_grad, u.full_grad.t)
-                self.coll.reduce_pushed(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq,
-                                        on_barrier=self._on_reduce_barrier)
+                self.coll.reduce_pushed(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq if last else None,
+                                        on_barrier=self._on_reduce_barrier, **acc)
                 self._push_pending = u.full_grad      # reusable after the NEXT flag round on this stream
             elif self._push_rs:
-                self.coll.reduce_scatter(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq,
-                                         on_barrier=self._on_reduce_barrier)
+                self.coll.reduce_scatter(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq if last else None,
+                                         on_barrier=self._on_reduce_barrier, **acc)
             else:
-                self.coll.reduce_scatter(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq)
+                self.coll.reduce_scatter(u.full_grad.t, u.grad_shard, 1.0 / W, self._gnorm_sq if last else None, **acc)
             if self.is_cuda and not getattr(u, "pushed", False):
                 u.full_grad.free_event.record(self.s_reduce)
         if m.shard_size > 1:
@@ -568,8 +591,38 @@ class ShardedModel(nn.Module):
         out = blk(*state)
         return self._as_tuple(out)
 
-    def _forward(self, tokens, labels=None, **head_kwargs):
+    def _begin_micro_step(self):
+        """Count one training micro-step (a forward with autograd on).  Returns True for the first micro-step of an
+        optimizer step, which resets the step-level state (||g||^2, clip coefficient)."""
+        k = self.grad_accum_steps
+        if k == 1:
+            self._micro = 1
+            return True
+        if self._micro >= k:
+            raise RuntimeError(f"grad_accum_steps={k}: {k} micro-steps have already run since the last optimizer step; "
+                               "call optimizer.step() before the next forward")
+        self._micro += 1
+        return self._micro == 1
+
+    def _check_accumulated(self, what: str):
+        k = self.grad_accum_steps
+        if k > 1 and self._micro != k:
+            raise RuntimeError(f"{what} after {self._micro} micro-step(s); grad_accum_steps={k} needs exactly {k} "
+                               "forward/backward micro-steps per optimizer step")
+
+    def optimizer_grad_scale(self) -> Optional[torch.Tensor]:
+        """Multiplier the fused AdamW applies to the gradient shard: the clip coefficient (None = not clipped) and, with
+        ``grad_accum_steps = k > 1``, the 1/k that turns the accumulated sum into the mean micro-batch gradient."""
+        self._check_accumulated("optimizer step")
+        if self.grad_accum_steps > 1 and self._clip_coef is None:
+            return self._inv_accum
+        return self._clip_coef
+
+    def _forward(self, tokens, labels=None, *, autograd_driven: bool = False, **head_kwargs):
+        """``autograd_driven``: the backward will come from ``loss.backward()`` (``forward``), with an upstream gradient
+        that may scale the loss, instead of from ``forward_backward``."""
         model, blocks = self.module, self.blocks
+        first = self._begin_micro_step() if torch.is_grad_enabled() else True
         fuse = self._fuse_gather and torch.is_grad_enabled()
         depth = 1 if fuse else self.prefetch_depth
         if self.is_cuda:
@@ -583,8 +636,9 @@ class ShardedModel(nn.Module):
                     self.coll.begin_step()             # ... on every rank (cross-GPU barrier, fused path)
         else:
             self.coll.begin_step()
-        self._gnorm_sq.zero_()
-        self._clip_coef = None
+        if first:
+            self._gnorm_sq.zero_()
+            self._clip_coef = None
         self._start_gather(self.root, fuse=False)
         if fuse and blocks:
             # block 0's own weights arrive INSIDE its first GEMM (QKV projection), consumed tile by tile
@@ -627,8 +681,12 @@ class ShardedModel(nn.Module):
                 if not keep:
                     self._release(u)
         head_in = self._detach_state(state, grad_on)
-        if grad_on:
-            self._prepare_grads(self.root)      # the head's dW is produced by the fused linear-CE of the forward
+        # the head's dW is produced by the fused linear-CE of the forward, straight into the bound gradient buffer.  Not so
+        # for an autograd-driven micro-step >= 2 on an unsharded mesh: that buffer already holds the earlier micro-steps,
+        # so the loss's upstream gradient could no longer scale this micro-step's dW alone.  The head then computes dW as
+        # an ordinary gradient; the backward binds the buffer (accumulating) and ``collect_grads`` adds it.
+        if grad_on and not (autograd_driven and self.mesh.shard_size == 1 and self._micro > 1):
+            self._prepare_grads(self.root)
         with torch.enable_grad() if grad_on else torch.no_grad():
             out = model.engine_head(*head_in, labels=labels, **head_kwargs) if labels is not None \
                 else model.engine_head(*head_in, **head_kwargs)
@@ -710,7 +768,8 @@ class ShardedModel(nn.Module):
 
     def forward_backward(self, tokens, labels, **head_kwargs) -> torch.Tensor:
         """One training micro-step: returns the (detached) mean loss; gradients end up reduced,
-        scaled by 1/world and sharded, with ||g||^2 accumulated for ``clip_grad_norm_``."""
+        scaled by 1/world and sharded, with ||g||^2 accumulated for ``clip_grad_norm_`` (on the last of
+        ``grad_accum_steps`` micro-steps; earlier ones add their gradient to the shard)."""
         loss = self._forward(tokens, labels, **head_kwargs)
         self._backward(None)
         return loss.detach()
@@ -721,14 +780,16 @@ class ShardedModel(nn.Module):
         reduced (all-reduce / reduce-scatter + replica reduce), scaled by 1/world and norm-accumulated."""
         if self.blocks:
             raise RuntimeError("forward_backward_custom is for root-only models")
+        first = self._begin_micro_step()
         if self.is_cuda:
             self.s_gather.wait_stream(self.s_compute)
             with torch.cuda.stream(self.s_gather):
                 self.coll.begin_step()
         else:
             self.coll.begin_step()
-        self._gnorm_sq.zero_()
-        self._clip_coef = None
+        if first:
+            self._gnorm_sq.zero_()
+            self._clip_coef = None
         self._start_gather(self.root, fuse=False)   # the step barrier above sits on the gather stream
         self._wait_gather(self.root)
         self._prepare_grads(self.root)
@@ -745,7 +806,7 @@ class ShardedModel(nn.Module):
     def forward(self, tokens, labels=None, **head_kwargs):
         if not torch.is_grad_enabled():
             return self._forward(tokens, labels, **head_kwargs)
-        out = self._forward(tokens, labels, **head_kwargs)
+        out = self._forward(tokens, labels, autograd_driven=True, **head_kwargs)
         return _EngineOutput.apply(self, out.detach(), self._anchor())
 
     def _anchor(self):
@@ -762,14 +823,20 @@ class ShardedModel(nn.Module):
         torch ``fully_sharded_data_parallel.py:1165-1215``, called at ``train_utils.py:96``)."""
         if norm_type != 2.0:
             raise NotImplementedError("only the L2 norm is supported")
+        self._check_accumulated("clip_grad_norm_")
+        k = self.grad_accum_steps
         total = self._gnorm_sq.clone()
         self.coll.all_reduce_scalar(total, over="shard")
         norm = total.sqrt()
+        if k > 1:
+            norm.div_(k)             # the shard holds the SUM of k micro-step gradients; the norm is that of their mean
         # engine-owned scalar: the asynchronous optimizer's kernels on ``s_opt`` read it after this call returns, so it
         # must not be a temporary the caching allocator could hand to the next step's compute-stream allocations
         if getattr(self, "_clip_coef_buf", None) is None:
             self._clip_coef_buf = torch.ones((), dtype=torch.float32, device=self.device)
         torch.clamp(max_norm / (norm + 1e-6), max=1.0, out=self._clip_coef_buf)
+        if k > 1:
+            self._clip_coef_buf.div_(k)   # AdamW's multiplier of the summed gradient: clip coefficient / k
         self._clip_coef = self._clip_coef_buf
         self.last_grad_norm = norm
         return norm

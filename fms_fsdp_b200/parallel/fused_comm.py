@@ -211,21 +211,24 @@ class FusedCollectives:
 
     # ---- gradient path ------------------------------------------------------------------------
     def reduce_scatter(self, full: torch.Tensor, shard32: torch.Tensor, scale: float, sumsq: Optional[torch.Tensor],
-                       on_barrier=None):
+                       on_barrier=None, accumulate: bool = False, replica: bool = True):
+        """``accumulate``: add into ``shard32`` instead of overwriting it; ``replica=False``: skip the HSDP replica
+        all-reduce (gradient accumulation runs it once, on the last micro-step)."""
         g = self.shard
         g.barrier(self.C, self._anchor, _SymGroup.CH_REDUCE)  # every rank's wgrads for this unit are complete
         if on_barrier is not None:
             on_barrier()
         hsdp = self.replica is not None or self._replica_nccl is not None
         self.C.reduce_scatter(g.table_of(full), shard32, g.index * shard32.numel(), g.size, g.index,
-                              full.dtype == torch.bfloat16, float(scale), None if hsdp else sumsq)
+                              full.dtype == torch.bfloat16, float(scale), None if hsdp else sumsq, 0, accumulate)
         if not hsdp:
             # results of this unit are final here; consumers need not wait for the trailing flag round
             self.last_reduce_done = torch.cuda.Event()
             self.last_reduce_done.record(torch.cuda.current_stream(self.device))
         g.barrier(self.C, self._anchor, _SymGroup.CH_REDUCE)  # peers are done reading my buffer before it is rewritten
         if hsdp:
-            self._replica_allreduce(shard32, sumsq)
+            if replica:
+                self._replica_allreduce(shard32, sumsq)
             self.last_reduce_done = None
 
     # ---- fused wgrad GEMM -> reduce-scatter (push) ----------------------------------------------------------------
@@ -239,11 +242,11 @@ class FusedCollectives:
         self.C.push_range(vec, g.table_of(staging), staging.numel() // g.size, 0, g.index)
 
     def reduce_pushed(self, staging: torch.Tensor, shard32: torch.Tensor, scale: float, sumsq: Optional[torch.Tensor],
-                      on_barrier=None):
+                      on_barrier=None, accumulate: bool = False, replica: bool = True):
         """After every rank pushed its wgrad tiles: ONE flag round (all tiles of all ranks have landed in my slots),
         then a LOCAL sum of the ``world`` slots.  There is no trailing barrier: a staging buffer is handed out again
         only after a LATER flag round on this stream has completed (``on_barrier`` lets the engine record that), which
-        implies every rank has finished summing it."""
+        implies every rank has finished summing it.  ``accumulate`` / ``replica``: as in ``reduce_scatter``."""
         g = self.shard
         n = shard32.numel()
         g.barrier(self.C, self._anchor, _SymGroup.CH_REDUCE)
@@ -257,9 +260,9 @@ class FusedCollectives:
             self._slice_tables[key] = tab
         hsdp = self.replica is not None or self._replica_nccl is not None
         self.C.reduce_scatter(tab, shard32, 0, g.size, 0, staging.dtype == torch.bfloat16, float(scale),
-                              None if hsdp else sumsq, self._slotsum_ctas)
+                              None if hsdp else sumsq, self._slotsum_ctas, accumulate)
         self.last_reduce_done = None
-        if hsdp:
+        if hsdp and replica:
             self._replica_allreduce(shard32, sumsq)
 
     def _replica_allreduce(self, shard32: torch.Tensor, sumsq: Optional[torch.Tensor]):

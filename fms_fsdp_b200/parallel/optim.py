@@ -31,10 +31,10 @@ class ShardedAdamW(torch.optim.Optimizer):
     def step(self, closure=None):
         loss = closure() if closure is not None else None
         g = self.param_groups[0]
+        eng = self.engine
+        coef = eng.optimizer_grad_scale()     # clip coefficient, and 1/k under gradient accumulation
         self._step += 1
         lr, (b1, b2), eps, wd = float(g["lr"]), g["betas"], g["eps"], g["weight_decay"]
-        eng = self.engine
-        coef = eng._clip_coef
 
         sharded_async = eng.async_optimizer and getattr(eng, "_async_sharded", False)
         epoch = eng._opt_epoch + 1 if sharded_async else 0
@@ -67,11 +67,13 @@ class ShardedAdamW(torch.optim.Optimizer):
         else:
             update_all()
         eng._clip_coef = None
+        eng._micro = 0
         eng.step_count = self._step
         return loss
 
     def zero_grad(self, set_to_none: bool = True):
-        # gradient buffers are overwritten (not accumulated) by every backward
+        # gradient buffers are overwritten by the first micro-step after a step (and accumulated over the others when
+        # the engine has ``grad_accum_steps > 1``): there is nothing to zero
         return None
 
     # flat, rank-local state (the Checkpointer uses the per-parameter sharded view instead)

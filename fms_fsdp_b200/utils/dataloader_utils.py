@@ -90,7 +90,9 @@ def get_data_loader(cfg, rank, world_size, postprocess=[causal_lm]):
     data = D.PreprocessDataset(data, torch.IntTensor)
     for p in postprocess:
         data = D.PreprocessDataset(data, p)
+    # the loader counts optimizer steps (batch_size x grad_accum_steps sequences each), so its state is written at the
+    # same steps as the model checkpoint
     data = D.CheckpointDataset(
         data, cfg.ckpt_load_path if cfg.resuming_dataset else cfg.ckpt_save_path,
-        cfg.checkpoint_interval, cfg.batch_size, cfg.ckpt_save_path)
+        cfg.checkpoint_interval, cfg.batch_size * getattr(cfg, "grad_accum_steps", 1), cfg.ckpt_save_path)
     return torch.utils.data.DataLoader(data, num_workers=cfg.num_workers, batch_size=cfg.batch_size)

@@ -7,7 +7,8 @@ recomputed?" answered before a job is queued.
 The numbers follow what the runtime allocates (``parallel/engine.py``) and what the autograd nodes of ``ops/functional.py`` save:
 
 * state, per parameter and divided by the shard-group size: fp32 master + bf16 shard + two fp32 AdamW moments (14 B) and the
-  fp32 gradient shard (4 B); unsharded (1 GPU / ddp) the gradient stays in the bf16 reduce dtype (2 B);
+  fp32 gradient shard (4 B); unsharded (1 GPU / ddp) the gradient stays in the bf16 reduce dtype (2 B), or fp32 (4 B) when
+  ``grad_accum_steps > 1`` accumulates micro-steps in it;
 * gathered parameters: ``prefetch + 1`` block-sized bf16 buffers and the root unit (embedding + head + final norm);
 * gradient staging (sharded only): ``push_pool`` block-sized buffers the wgrad GEMMs of all ranks push into, plus the root
   unit's unsharded gradient (pull path);
@@ -63,7 +64,8 @@ def _recomputed_blocks(nlayers: int, selective_checkpointing, enabled: bool) -> 
 
 def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp", hsdp_shard_size: int = 0,
                batch_size: int = 2, seq_length: int = 4096, fsdp_activation_checkpointing: bool = False,
-               selective_checkpointing="1", prefetch: int = 1, push_pool: int = 3, ce_chunk_rows: int = 4096) -> MemoryPlan:
+               selective_checkpointing="1", prefetch: int = 1, push_pool: int = 3, ce_chunk_rows: int = 4096,
+               grad_accum_steps: int = 1) -> MemoryPlan:
     from fms_fsdp_b200.parallel.mesh import resolve_shard_size
     from fms_fsdp_b200.utils.config_utils import get_model_config
 
@@ -79,7 +81,10 @@ def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp
 
     parts: Dict[str, float] = {}
     parts["master + bf16 shard + AdamW moments (14 B/param / shard)"] = 14.0 * n_params / S / GiB
-    parts["gradient shard (fp32; bf16 when unsharded)"] = (4.0 if S > 1 else 2.0) * n_params / S / GiB
+    if grad_accum_steps > 1:
+        parts["gradient shard (fp32, accumulates micro-steps)"] = 4.0 * n_params / S / GiB
+    else:
+        parts["gradient shard (fp32; bf16 when unsharded)"] = (4.0 if S > 1 else 2.0) * n_params / S / GiB
     if S > 1:
         parts[f"gathered parameters ({prefetch + 1} blocks + root, bf16)"] = 2.0 * ((prefetch + 1) * block_params + root_params) / GiB
         parts[f"gradient staging ({push_pool} block buffers + root, bf16)"] = 2.0 * (push_pool * block_params + root_params) / GiB

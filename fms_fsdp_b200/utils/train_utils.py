@@ -254,14 +254,30 @@ class _LossReadback:
         return done
 
 
+def _step_groups(loader, k: int):
+    """Consecutive groups of ``k`` loader batches: the micro-batches of one optimizer step."""
+    group = []
+    for batch in loader:
+        group.append(batch)
+        if len(group) == k:
+            yield group
+            group = []
+
+
 def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, profiler, checkpointer,
           start_step, tokens_seen):
-    """Reference: ``fms_fsdp/utils/train_utils.py:21-180``."""
+    """Reference: ``fms_fsdp/utils/train_utils.py:21-180``.
+
+    ``cfg.grad_accum_steps = k`` draws k loader batches per optimizer step (the engine averages their gradients).
+    Steps, the LR schedule, report / checkpoint intervals and ``fault_inject_step`` count optimizer steps; the reported
+    loss is the mean of the k micro-batch losses and token counts include all k micro-batches."""
     tracker_fn = _init_tracker(cfg, rank)
     is_cuda = torch.cuda.is_available() and getattr(model, "is_cuda", True)
     device = getattr(model, "device", torch.device("cuda", local_rank) if is_cuda else torch.device("cpu"))
     world_size = int(os.environ.get("WORLD_SIZE", 1))
     engine_mode = hasattr(model, "forward_backward")
+    accum = int(getattr(cfg, "grad_accum_steps", 1))
+    step_tokens = cfg.batch_size * cfg.seq_length * accum     # per GPU and optimizer step
     model.train()
     ddp_stats = torch.zeros(3, device=device)  # [sum loss, sum gnorm, steps]
     to_device = _H2DStager(device)
@@ -280,25 +296,31 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
     start = loop_start = time.time()
     train_loss = -1
     new_tokens_seen = 0
-    for batch_idx, (input, label) in enumerate(train_loader, start=start_step + 1):
+    for batch_idx, micro_batches in enumerate(_step_groups(train_loader, accum), start=start_step + 1):
         if batch_idx > cfg.num_steps:
             break
         if cfg.fault_inject_step and batch_idx == cfg.fault_inject_step and rank == min(1, world_size - 1):
             print(f"[fault-inject] rank {rank} exiting at step {batch_idx}", flush=True)
             os._exit(17)
-        input = to_device(input)
-        label = to_device(label)
 
         optimizer.zero_grad()
-        if engine_mode and cfg.fused_cross_entropy:
-            loss = model.forward_backward(input, label.long() if label.dtype != torch.long else label)
-        else:
-            output = model(input)
-            output = output.logits if hasattr(output, "logits") else output
-            loss = torch.nn.functional.cross_entropy(output.view(-1, output.size(-1)).float(), label.view(-1).long())
-            del output
-            loss.backward()
-            loss = loss.detach()
+        loss = None
+        for input, label in micro_batches:
+            input = to_device(input)
+            label = to_device(label)
+            if engine_mode and cfg.fused_cross_entropy:
+                micro_loss = model.forward_backward(input, label.long() if label.dtype != torch.long else label)
+            else:
+                output = model(input)
+                output = output.logits if hasattr(output, "logits") else output
+                micro_loss = torch.nn.functional.cross_entropy(output.view(-1, output.size(-1)).float(),
+                                                               label.view(-1).long())
+                del output
+                micro_loss.backward()
+                micro_loss = micro_loss.detach()
+            loss = micro_loss if loss is None else loss + micro_loss
+        if accum > 1:
+            loss = loss / accum
         gnorm = model.clip_grad_norm_(cfg.grad_clip_thresh)
         optimizer.step()
         scheduler.step()
@@ -318,7 +340,7 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
         if profiler:
             profiler.step()
 
-        new_tokens_seen = (batch_idx - start_step) * world_size * cfg.batch_size * cfg.seq_length
+        new_tokens_seen = (batch_idx - start_step) * world_size * step_tokens
         if batch_idx % cfg.report_interval == 0:
             dev_step_time = None
             if is_cuda:
@@ -349,8 +371,8 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 current_gnorm = g_norm.item()
                 current_step_time = (time.time() - start) / cfg.report_interval
                 overall_step_time = elapsed_time / (batch_idx - start_step)
-                current_throughput = int(cfg.batch_size * cfg.seq_length / current_step_time)
-                overall_throughput = int(cfg.batch_size * cfg.seq_length / overall_step_time)
+                current_throughput = int(step_tokens / current_step_time)
+                overall_throughput = int(step_tokens / overall_step_time)
                 reserved_mem = torch.cuda.max_memory_reserved(device) if is_cuda else 0
                 allocated_mem = torch.cuda.max_memory_allocated(device) if is_cuda else 0
                 print("step:", batch_idx)
@@ -368,7 +390,7 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 if dev_step_time is not None:
                     print("device step time (max over ranks):", dev_step_time)
                     if flops_tok is not None:
-                        tf = cfg.batch_size * cfg.seq_length / dev_step_time * flops_tok / 1e12
+                        tf = step_tokens / dev_step_time * flops_tok / 1e12
                         print("model TFLOP/s per gpu:", round(tf, 1), " MFU vs measured bf16 peak:",
                               round(tf / peak_tflops(), 4))
                 sys.stdout.flush()

@@ -91,6 +91,7 @@ def main(**kwargs):
         param_init_fn=param_init_fn,
         auto_wrap_policy=wrapping_policy,
         local_world=(torch.cuda.device_count() if use_cuda else None),
+        grad_accum_steps=cfg.grad_accum_steps,
     )
     model.poison_released_params = bool(cfg.poison_released_params) or model.poison_released_params
     if rank == 0:
