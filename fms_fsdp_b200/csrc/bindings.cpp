@@ -63,6 +63,7 @@ DECL int b200_attn_bwd(const void*, const void*, const void*, const float*, void
                        float, const float*, cudaStream_t, const int*);
 DECL void b200_gemm2_set_rope(const float*, int, int, int);
 DECL void b200_gemm2_set_swiglu(void*, int, int, int);
+DECL void b200_gemm2_set_tile(int);
 DECL int b200_gemm2_fp8(const void*, const void*, void*, const float*, const float*, int, int, int, int, int, int, cudaStream_t);
 DECL int b200_quant_rowwise_e4m3(const void*, void*, float*, int, int, int, int, cudaStream_t);
 DECL void b200_gemm2_set_push(void* const*, long long, long long, int, int, int);
@@ -830,6 +831,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("ssd_scan_bwd", &ssd_scan_bwd);
   m.def("set_gemm_2cta", &set_gemm_2cta);
   m.def("get_gemm_2cta", &get_gemm_2cta);
+  // private: pins the tile of the single-GPU GEMMs (0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256) so that the
+  // GEMM benchmark and the tests can compare both tiles on the same operands
+  m.def("_set_gemm_tile", [](int64_t mode) { b200_gemm2_set_tile((int)mode); });
   m.def("gemm_ag", &gemm_ag);
   m.def("gemm_push", &gemm_push);
   m.def("quant_rowwise_e4m3", &quant_rowwise_e4m3);

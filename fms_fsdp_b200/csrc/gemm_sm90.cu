@@ -13,6 +13,9 @@
 //
 // Warp roles (384 threads): warpgroup 0 = producer (warp 0 lane 0 issues TMA; warps 2-3 are the comm warps of the fused
 // all-gather), warpgroups 1-2 = consumers (wgmma + epilogue).
+//
+// gemm_wide_bf16 is the same pipeline on a 128 x 256 tile (wgmma m64n256k16) for the GEMMs without fused communication;
+// use_wide picks the tile per launch.
 #include "common.cuh"
 #include "tensormap.h"
 #include "wgmma.cuh"
@@ -196,6 +199,59 @@ B200_DEVINL void epi_pair(const GemmParams& p, OutT* crow, int row, int col, flo
     f0 += r.x; f1 += r.y;
   }
   store2(crow + col, f0, f1);
+}
+
+// Register epilogue of one consumer warpgroup's 64-row slice of a tile that is 8 * NJ columns wide (NJ = 16: 128x128
+// kernel, 32: 128x256 kernel) in tile column nt.  The thread holds rows rbase and rbase + 8, column pairs 8 j + cq for
+// j < NJ.  EPI_SWIGLU: the tile holds gate and up of 4 * NJ features side by side.
+template <int EPI, typename OutT, int NJ>
+B200_DEVINL void epilogue_tile(const GemmParams& p, const float (&acc)[4 * NJ], size_t boff, int rbase, int nt, int cq) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = rbase + 8 * h;
+    if (row >= p.M) continue;
+    OutT* crow = reinterpret_cast<OutT*>(p.C) + boff + static_cast<size_t>(row) * p.ldc;
+    if constexpr (EPI == EPI_SWIGLU) {
+      __nv_bfloat16* arow = reinterpret_cast<__nv_bfloat16*>(p.aux) + static_cast<size_t>(row) * p.ld_aux;
+#pragma unroll
+      for (int j = 0; j < NJ / 2; ++j) {
+        const int col = nt * (4 * NJ) + 8 * j + cq;
+        const uint32_t w1 = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        const uint32_t w2 = pack_bf16x2(acc[4 * (j + NJ / 2) + 2 * h], acc[4 * (j + NJ / 2) + 2 * h + 1]);
+        // activation from the ROUNDED projection: forward and backward see the same gate / up values
+        const float2 x1 = unpack_bf16x2(w1), x2 = unpack_bf16x2(w2);
+        const float2 gt = p.swi_gate_first ? x1 : x2, up = p.swi_gate_first ? x2 : x1;
+        *reinterpret_cast<uint32_t*>(crow + col) = w1;
+        *reinterpret_cast<uint32_t*>(crow + p.swi_F + col) = w2;
+        *reinterpret_cast<uint32_t*>(arow + col) =
+            pack_bf16x2(gt.x * sigmoidf_fast(gt.x) * up.x, gt.y * sigmoidf_fast(gt.y) * up.y);
+      }
+    } else if constexpr (EPI == EPI_SWIGLU_BWD) {
+      const __nv_bfloat16* grow = reinterpret_cast<const __nv_bfloat16*>(p.aux) + static_cast<size_t>(row) * p.ld_aux;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const int col = nt * (8 * NJ) + 8 * j + cq;
+        if (col >= p.N) break;
+        const float2 x1 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + col));
+        const float2 x2 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + p.swi_F + col));
+        const float2 gt = p.swi_gate_first ? x1 : x2, up = p.swi_gate_first ? x2 : x1;
+        const float ds0 = acc[4 * j + 2 * h], ds1 = acc[4 * j + 2 * h + 1];
+        const float s0 = sigmoidf_fast(gt.x), s1 = sigmoidf_fast(gt.y);
+        const float dg0 = ds0 * up.x * s0 * (1.f + gt.x * (1.f - s0)), dg1 = ds1 * up.y * s1 * (1.f + gt.y * (1.f - s1));
+        const float du0 = ds0 * gt.x * s0, du1 = ds1 * gt.y * s1;
+        const uint32_t pg = pack_bf16x2(dg0, dg1), pu = pack_bf16x2(du0, du1);
+        *reinterpret_cast<uint32_t*>(crow + col) = p.swi_gate_first ? pg : pu;
+        *reinterpret_cast<uint32_t*>(crow + p.swi_F + col) = p.swi_gate_first ? pu : pg;
+      }
+    } else {
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const int col = nt * (8 * NJ) + 8 * j + cq;
+        if (col >= p.N) break;
+        epi_pair<EPI, OutT>(p, crow, row, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+      }
+    }
+  }
 }
 
 template <bool A_MN, bool B_MN, int EPI, typename OutT, bool AG, bool FP8 = false, bool BATCH = false>
@@ -411,52 +467,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           continue;
         }
       }
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int row = rbase + 8 * h;
-        if (row >= p.M) continue;
-        OutT* crow = reinterpret_cast<OutT*>(p.C) + boff + static_cast<size_t>(row) * p.ldc;
-        if constexpr (EPI == EPI_SWIGLU) {
-          __nv_bfloat16* arow = reinterpret_cast<__nv_bfloat16*>(p.aux) + static_cast<size_t>(row) * p.ld_aux;
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int col = nt * 64 + 8 * j + cq;
-            const uint32_t w1 = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-            const uint32_t w2 = pack_bf16x2(acc[4 * (j + 8) + 2 * h], acc[4 * (j + 8) + 2 * h + 1]);
-            // activation from the ROUNDED projection: forward and backward see the same gate / up values
-            const float2 x1 = unpack_bf16x2(w1), x2 = unpack_bf16x2(w2);
-            const float2 gt = p.swi_gate_first ? x1 : x2, up = p.swi_gate_first ? x2 : x1;
-            *reinterpret_cast<uint32_t*>(crow + col) = w1;
-            *reinterpret_cast<uint32_t*>(crow + p.swi_F + col) = w2;
-            *reinterpret_cast<uint32_t*>(arow + col) =
-                pack_bf16x2(gt.x * sigmoidf_fast(gt.x) * up.x, gt.y * sigmoidf_fast(gt.y) * up.y);
-          }
-        } else if constexpr (EPI == EPI_SWIGLU_BWD) {
-          const __nv_bfloat16* grow = reinterpret_cast<const __nv_bfloat16*>(p.aux) + static_cast<size_t>(row) * p.ld_aux;
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int col = nt * BN + 8 * j + cq;
-            if (col >= p.N) break;
-            const float2 x1 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + col));
-            const float2 x2 = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(grow + p.swi_F + col));
-            const float2 gt = p.swi_gate_first ? x1 : x2, up = p.swi_gate_first ? x2 : x1;
-            const float ds0 = acc[4 * j + 2 * h], ds1 = acc[4 * j + 2 * h + 1];
-            const float s0 = sigmoidf_fast(gt.x), s1 = sigmoidf_fast(gt.y);
-            const float dg0 = ds0 * up.x * s0 * (1.f + gt.x * (1.f - s0)), dg1 = ds1 * up.y * s1 * (1.f + gt.y * (1.f - s1));
-            const float du0 = ds0 * gt.x * s0, du1 = ds1 * gt.y * s1;
-            const uint32_t pg = pack_bf16x2(dg0, dg1), pu = pack_bf16x2(du0, du1);
-            *reinterpret_cast<uint32_t*>(crow + col) = p.swi_gate_first ? pg : pu;
-            *reinterpret_cast<uint32_t*>(crow + p.swi_F + col) = p.swi_gate_first ? pu : pg;
-          }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int col = nt * BN + 8 * j + cq;
-            if (col >= p.N) break;
-            epi_pair<EPI, OutT>(p, crow, row, col, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-          }
-        }
-      }
+      epilogue_tile<EPI, OutT, BN / 8>(p, acc, boff, rbase, nt, cq);
     }
     if constexpr (EPI == EPI_PUSH) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // every pushed row is out
   }
@@ -480,18 +491,174 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
   return (int)cudaGetLastError();
 }
 
+// ---- 128 x 256 tile ("wide"), for the GEMMs without fused communication.  The same pipeline with twice the B tile per
+// stage: a k-block moves 48 KiB for 4.2 MFLOP (85 FLOP per byte from L2, against 64 for 128 x 128), and each consumer
+// warpgroup issues m64n256k16, which reads 10 KiB of shared-memory operands per 524k FLOP where two m64n128k16 read
+// 12 KiB.  A 64 x 256 fp32 accumulator is 128 registers per consumer thread, more than 384 threads get by default:
+// setmaxnreg hands the producer warpgroup's registers to the consumers (128 x 40 + 256 x 232 <= 64K).
+// Epilogues: store, +residual, accumulate (bf16 or fp32 output), RoPE, SwiGLU forward (F % 128 == 0) and backward.
+constexpr int WBN = 256;
+constexpr int W_STAGES = 4;
+constexpr int W_STAGE_BYTES = A_BYTES + WBN * BK * 2;   // 16 + 32 KiB
+constexpr int W_SMEM_BYTES = W_STAGES * W_STAGE_BYTES + 1024 + 256;
+
+template <int N>
+B200_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+B200_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
+template <bool A_MN, bool B_MN, int EPI, typename OutT>
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wide_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + W_STAGES * W_STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + W_STAGES;
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_kb = (p.K + BK - 1) / BK;
+  const int num_tiles = p.m_tiles * p.n_tiles;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int s = 0; s < W_STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ============================== TMA producer ==============================
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+        int mt, nt;
+        tile_coords(t, p.m_tiles, p.n_tiles, mt, nt);
+        const int m0 = mt * BM;
+        // first B row (K-major) or column (MN-major) of the tile; SwiGLU: 128 features of the first half of the fused
+        // weight in B rows [f0, f0 + 128), the same features of the second half in [F + f0, F + f0 + 128)
+        const int n0 = (EPI == EPI_SWIGLU) ? nt * 128 : nt * WBN;
+        const int n2 = (EPI == EPI_SWIGLU) ? n0 + p.swi_F : n0 + 128;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * W_STAGE_BYTES;
+          uint8_t* sb = sa + A_BYTES;
+          const int k0 = kb * BK;
+          mbar_arrive_expect_tx(&full_bar[stage], W_STAGE_BYTES);
+          if constexpr (!A_MN) {
+            tma_load_2d(sa, &tmA, &full_bar[stage], k0, m0);                     // box {64 k, 128 rows}
+          } else {
+            tma_load_2d(sa, &tmA, &full_bar[stage], m0, k0);                     // boxes {64 m, 64 k-rows}
+            tma_load_2d(sa + 64 * BK * 2, &tmA, &full_bar[stage], m0 + 64, k0);
+          }
+#pragma unroll
+          for (int q = 0; q < 4; ++q) {                                            // four 64-wide quarters of B
+            const int nq = (q < 2 ? n0 : n2) + 64 * (q & 1);
+            if constexpr (!B_MN) tma_load_2d(sb + q * 64 * BK * 2, &tmB, &full_bar[stage], k0, nq);
+            else                 tma_load_2d(sb + q * 64 * BK * 2, &tmB, &full_bar[stage], nq, k0);
+          }
+          if (++stage == W_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ============================== consumers: wgmma + epilogue ==============================
+    const int cw = (warp >> 2) - 1;          // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
+    const int w4 = warp & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+      int mt, nt;
+      tile_coords(t, p.m_tiles, p.n_tiles, mt, nt);
+      float acc[128];
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_u32(smem + stage * W_STAGE_BYTES) + cw * (64 * 128);
+        const uint32_t sb = smem_u32(smem + stage * W_STAGE_BYTES) + A_BYTES;
+        const uint64_t a0 = make_smem_desc(sa, 0, 1024);
+        const uint64_t bd0 = make_smem_desc(sb, B_MN ? 64 * BK * 2 : 0, 1024);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k) {
+          const uint64_t adesc = a0 + ((A_MN ? k * 2048 : k * 32) >> 4);
+          const uint64_t bdesc = bd0 + ((B_MN ? k * 2048 : k * 32) >> 4);
+          wgmma_bf16_ss_n256<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb | k) != 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                     // the previous k-block's MMAs have retired: release its stage
+        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        if (++stage == W_STAGES) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      const int rbase = mt * BM + cw * 64 + w4 * 16 + (lane >> 2);
+      epilogue_tile<EPI, OutT, WBN / 8>(p, acc, 0, rbase, nt, 2 * (lane & 3));
+    }
+  }
+}
+
+template <bool A_MN, bool B_MN, int EPI, typename OutT>
+static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
+  auto kern = gemm_wide_bf16<A_MN, B_MN, EPI, OutT>;
+  static bool configured = false;
+  if (!configured) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM_BYTES);
+    if (e != cudaSuccess) return (int)e;
+    configured = true;
+  }
+  p.n_tiles = (EPI == EPI_SWIGLU) ? p.swi_F / 128 : (p.N + WBN - 1) / WBN;
+  const long long tiles = (long long)p.m_tiles * p.n_tiles;
+  const int grid = tiles < sm_count() ? (int)tiles : sm_count();
+  kern<<<grid, THREADS, W_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  return (int)cudaGetLastError();
+}
+
+// 0: the launcher picks the tile; 1: always 128 x 128; 2: 128 x 256 wherever the epilogue allows it.  Set only by the
+// GEMM benchmark and the tests, which compare the two tiles on the same operands.
+static int g_tile_override = 0;
+
+// The wide tile moves less data per FLOP but halves the tile count, so it wins unless it leaves a worse last wave:
+// a persistent sweep takes about ceil(tiles / SMs) tile times, and a wide tile takes WIDE_TILE_COST / 16 of two narrow
+// ones.
+constexpr int WIDE_TILE_COST = 15;
+static bool use_wide(const GemmParams& p, int epi) {
+  if (g_tile_override == 1 || (epi == EPI_SWIGLU && p.swi_F % 128)) return false;
+  if (g_tile_override == 2) return true;
+  const long long sm = sm_count();
+  const long long n_wide = (epi == EPI_SWIGLU) ? p.swi_F / 128 : (p.N + WBN - 1) / WBN;
+  const long long waves_narrow = ((long long)p.m_tiles * p.n_tiles + sm - 1) / sm;
+  const long long waves_wide = ((long long)p.m_tiles * n_wide + sm - 1) / sm;
+  return 2 * WIDE_TILE_COST * waves_wide <= 16 * waves_narrow;
+}
+
+// every GEMM of the single-GPU path (no fused all-gather, no push): one launch of the tile use_wide picks
+template <bool A_MN, bool B_MN, int EPI, typename OutT>
+static int launch_local(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
+  if (use_wide(p, EPI)) return launch_wide<A_MN, B_MN, EPI, OutT>(tmA, tmB, p, stream);
+  return launch<A_MN, B_MN, EPI, OutT, false>(tmA, tmB, p, AgParams{}, stream);
+}
+
 template <bool A_MN, bool B_MN>
 static int dispatch_epi(const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int epi, int out_fp32,
                         cudaStream_t s) {
-  const AgParams ag{};
   if (out_fp32) {
-    if (epi == EPI_STORE) return launch<A_MN, B_MN, EPI_STORE, float, false>(a, b, p, ag, s);
-    if (epi == EPI_RESIDUAL) return launch<A_MN, B_MN, EPI_RESIDUAL, float, false>(a, b, p, ag, s);
-    return launch<A_MN, B_MN, EPI_ACCUM, float, false>(a, b, p, ag, s);
+    if (epi == EPI_STORE) return launch_local<A_MN, B_MN, EPI_STORE, float>(a, b, p, s);
+    if (epi == EPI_RESIDUAL) return launch_local<A_MN, B_MN, EPI_RESIDUAL, float>(a, b, p, s);
+    return launch_local<A_MN, B_MN, EPI_ACCUM, float>(a, b, p, s);
   }
-  if (epi == EPI_STORE) return launch<A_MN, B_MN, EPI_STORE, __nv_bfloat16, false>(a, b, p, ag, s);
-  if (epi == EPI_RESIDUAL) return launch<A_MN, B_MN, EPI_RESIDUAL, __nv_bfloat16, false>(a, b, p, ag, s);
-  return launch<A_MN, B_MN, EPI_ACCUM, __nv_bfloat16, false>(a, b, p, ag, s);
+  if (epi == EPI_STORE) return launch_local<A_MN, B_MN, EPI_STORE, __nv_bfloat16>(a, b, p, s);
+  if (epi == EPI_RESIDUAL) return launch_local<A_MN, B_MN, EPI_RESIDUAL, __nv_bfloat16>(a, b, p, s);
+  return launch_local<A_MN, B_MN, EPI_ACCUM, __nv_bfloat16>(a, b, p, s);
 }
 
 // batched dispatch: store / accumulate epilogues, bf16 or fp32 output
@@ -577,6 +744,9 @@ extern "C" void b200_gemm2_set_swiglu(void* aux, int ld_aux, int F, int gate_fir
   b200::g_swi_aux = aux; b200::g_swi_ld = ld_aux; b200::g_swi_F = F; b200::g_swi_gate_first = gate_first;
 }
 
+// tile of the single-GPU GEMMs: 0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256 where the epilogue allows it
+extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode == 1 || mode == 2) ? mode : 0; }
+
 // C[M,N] = op(A) op(B) (+R | +C | fused epilogue).  a_mn: A is stored [K,M] (M contiguous) else [M,K];  b_mn: B is
 // stored [K,N] (N contiguous) else [N,K].  lda/ldb/ldc/ldr are row strides in elements.  Returns 0 or an error code.
 extern "C" int b200_gemm2_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda,
@@ -586,25 +756,24 @@ extern "C" int b200_gemm2_bf16(const void* A, const void* B, void* C, const void
   CUtensorMap tmA, tmB;
   if (int rc = make_maps(&tmA, &tmB, A, B, M, N, K, lda, ldb, a_mn, b_mn)) return rc;
   GemmParams p = make_params(C, R, M, N, K, ldc, ldr, epi);
-  const AgParams ag{};
   if (epi == EPI_SWIGLU) {   // nt; N = 2F rows of the fused weight, tiles of 64 features
     if (a_mn || b_mn || out_fp32 || !p.aux || p.swi_F <= 0 || N != 2 * p.swi_F || (p.swi_F % 64) || (p.ld_aux % 8)) return -11;
     p.N = p.swi_F;
     p.n_tiles = p.swi_F / 64;
-    return launch<false, false, EPI_SWIGLU, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    return launch_local<false, false, EPI_SWIGLU, __nv_bfloat16>(tmA, tmB, p, stream);
   }
   if (epi == EPI_SWIGLU_BWD) {   // nn; N = F columns of dS, output [M, 2F]
     if (a_mn || !b_mn || out_fp32 || !p.aux || p.swi_F != N || (N % 8) || (p.ld_aux % 8)) return -12;
-    return launch<false, true, EPI_SWIGLU_BWD, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    return launch_local<false, true, EPI_SWIGLU_BWD, __nv_bfloat16>(tmA, tmB, p, stream);
   }
   if (epi == EPI_ROPE) {
     if (a_mn || b_mn || out_fp32 || !p.rope || (p.rope_hd % 8) || (p.rope_cols % 8)) return -8;
-    return launch<false, false, EPI_ROPE, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    return launch_local<false, false, EPI_ROPE, __nv_bfloat16>(tmA, tmB, p, stream);
   }
   if (epi == EPI_PUSH) {   // wgrad (tn) only; every 8-element vector must stay inside one owner's slice
     if (!a_mn || !b_mn || out_fp32 || !p.push_bases || p.push_n <= 0 || (p.push_n % 8) || (p.push_off % 8) || (ldc % 8))
       return -9;
-    return launch<true, true, EPI_PUSH, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    return launch<true, true, EPI_PUSH, __nv_bfloat16, false>(tmA, tmB, p, AgParams{}, stream);
   }
   if (a_mn) {
     if (b_mn) return dispatch_epi<true, true>(tmA, tmB, p, epi, out_fp32, stream);
