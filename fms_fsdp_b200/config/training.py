@@ -108,4 +108,5 @@ class train_config:
     poison_released_params: bool = False     # debug: NaN-fill a unit's gathered parameters on release (use-after-free trap)
     grad_dtype: str = "bf16"                 # dtype of the unsharded gradient buffer (reference reduce_dtype=bf16)
     document_attention_mask: bool = False    # Llama: attention stops at eos_token in packed lines (RoPE positions are not reset)
+    qk_norm: bool = False                    # Llama: per-head RMSNorm of q and k before RoPE (Qwen3 QK-norm), for any variant
     grad_accum_steps: int = 1                # micro-batches per optimizer step (global batch = world x batch_size x this)

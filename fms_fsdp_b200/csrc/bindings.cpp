@@ -49,6 +49,11 @@ DECL int b200_rmsnorm_bwd_f32(const void*, const float*, const void*, const floa
 DECL int b200_rmsnorm_gated_fwd(const void*, const void*, const void*, void*, float*, int, int, float, cudaStream_t);
 DECL int b200_rmsnorm_gated_bwd(const void*, const void*, const void*, const void*, const float*, void*, void*, float*, float*, int, int, cudaStream_t);
 DECL int b200_rope(void*, const float*, int, int, int, int, int, int, int, int, int, cudaStream_t);
+DECL int b200_qk_norm_rope(void*, void*, float*, const void*, const void*, const float*, int, int, int, int, int, int, float,
+                           cudaStream_t);
+DECL int b200_qk_norm_bwd_grid(int, int, int);
+DECL int b200_qk_norm_bwd(void*, const void*, const float*, const void*, const void*, float*, float*, int, int, int, int,
+                          int, cudaStream_t);
 DECL int b200_swiglu_fwd(const void*, void*, long long, int, int, cudaStream_t);
 DECL int b200_swiglu_bwd(const void*, const void*, void*, long long, int, int, cudaStream_t);
 DECL int b200_embedding_fwd(const void*, int, const void*, void*, long long, int, cudaStream_t);
@@ -253,6 +258,50 @@ void rope(at::Tensor& qkv, const at::Tensor& table, int64_t seq_len, int64_t nro
   TORCH_CHECK(table.size(0) >= seq_len + pos_offset && table.size(1) == rot / 2, "rope table too small");
   check(b200_rope(qkv.data_ptr(), table.data_ptr<float>(), qkv.size(0), seq_len, qkv.stride(0), nrot_heads, hd, rot,
                   inverse, pos_offset, interleaved, cur_stream()), "rope");
+}
+// QK-norm + RoPE in place on the q / k heads of qkv [M, (H + 2 KVH) * hd]; returns the pre-norm q / k
+// [M, (H + KVH) * hd] and rstd [M, H + KVH] the backward needs.
+std::vector<at::Tensor> qk_norm_rope(at::Tensor& qkv, const at::Tensor& wq, const at::Tensor& wk, const at::Tensor& table,
+                                     int64_t seq_len, int64_t H, int64_t KVH, int64_t hd, double eps) {
+  c10::cuda::CUDAGuard guard(qkv.device());
+  need(qkv, "qkv", at::kBFloat16);
+  need(wq, "w_q", at::kBFloat16);
+  need(wk, "w_k", at::kBFloat16);
+  need(table, "table", at::kFloat);
+  need_rowmajor2d(qkv, "qkv");
+  TORCH_CHECK(wq.is_contiguous() && wk.is_contiguous() && wq.numel() == hd && wk.numel() == hd, "qk_norm: weights must be [hd]");
+  TORCH_CHECK(qkv.size(1) == (H + 2 * KVH) * hd && H % KVH == 0, "qk_norm: qkv width != (H + 2 KVH) * hd");
+  TORCH_CHECK(table.is_contiguous() && table.size(0) >= seq_len && table.size(1) == hd / 2, "rope table too small");
+  const int M = qkv.size(0);
+  TORCH_CHECK(M % seq_len == 0, "qk_norm: rows must be whole sequences");
+  auto xqk = at::empty({M, (H + KVH) * hd}, qkv.options());
+  auto rstd = at::empty({M, H + KVH}, qkv.options().dtype(at::kFloat));
+  check(b200_qk_norm_rope(qkv.data_ptr(), xqk.data_ptr(), rstd.data_ptr<float>(), wq.data_ptr(), wk.data_ptr(),
+                          table.data_ptr<float>(), M, (int)seq_len, qkv.stride(0), (int)H, (int)KVH, (int)hd, (float)eps,
+                          cur_stream()), "qk_norm_rope");
+  return {xqk, rstd};
+}
+// in place on the q / k heads of dqkv; returns fp32 (dw_q, dw_k)
+std::vector<at::Tensor> qk_norm_bwd(at::Tensor& dqkv, const at::Tensor& xqk, const at::Tensor& rstd, const at::Tensor& wq,
+                                    const at::Tensor& wk, int64_t H, int64_t KVH, int64_t hd) {
+  c10::cuda::CUDAGuard guard(dqkv.device());
+  need(dqkv, "dqkv", at::kBFloat16);
+  need(xqk, "xqk", at::kBFloat16);
+  need(rstd, "rstd", at::kFloat);
+  need(wq, "w_q", at::kBFloat16);
+  need(wk, "w_k", at::kBFloat16);
+  need_rowmajor2d(dqkv, "dqkv");
+  TORCH_CHECK(wq.is_contiguous() && wk.is_contiguous() && wq.numel() == hd && wk.numel() == hd, "qk_norm: weights must be [hd]");
+  TORCH_CHECK(dqkv.size(1) == (H + 2 * KVH) * hd, "qk_norm_bwd: dqkv width != (H + 2 KVH) * hd");
+  const int M = dqkv.size(0);
+  TORCH_CHECK(xqk.is_contiguous() && xqk.numel() == (int64_t)M * (H + KVH) * hd, "qk_norm_bwd: xqk shape");
+  TORCH_CHECK(rstd.is_contiguous() && rstd.numel() == (int64_t)M * (H + KVH), "qk_norm_bwd: rstd shape");
+  auto part = at::empty({b200_qk_norm_bwd_grid(M, (int)(H + KVH), (int)hd), 2 * hd}, rstd.options());
+  auto dw = at::empty({2, hd}, rstd.options());
+  check(b200_qk_norm_bwd(dqkv.data_ptr(), xqk.data_ptr(), rstd.data_ptr<float>(), wq.data_ptr(), wk.data_ptr(),
+                         part.data_ptr<float>(), dw.data_ptr<float>(), M, dqkv.stride(0), (int)H, (int)KVH, (int)hd,
+                         cur_stream()), "qk_norm_bwd", 2);
+  return {dw[0], dw[1]};
 }
 at::Tensor swiglu_fwd(const at::Tensor& gu, bool gate_first) {
   c10::cuda::CUDAGuard guard(gu.device());
@@ -775,6 +824,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rmsnorm_gated_fwd", &rmsnorm_gated_fwd);
   m.def("rmsnorm_gated_bwd", &rmsnorm_gated_bwd);
   m.def("rope", &rope);
+  m.def("qk_norm_rope", &qk_norm_rope);
+  m.def("qk_norm_bwd", &qk_norm_bwd);
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("embedding_fwd", &embedding_fwd);

@@ -723,6 +723,123 @@ __global__ void sumsq_kernel(const T* __restrict__ x, size_t n, float* __restric
   if (threadIdx.x == 0) atomicAdd(out, s);
 }
 
+// ------------------------------------------------------------------------------------ QK-norm + RoPE
+// Per-head RMSNorm of the q and k heads of a fused [M, (H + 2 KVH) * hd] projection (Qwen3 / OLMo-style QK-norm),
+// followed by the interleaved-pair RoPE, in place.  Work item = one (row, head) of the H + KVH rotated heads, held by a
+// group of G = hd / 8 lanes (one 16-byte vector each); the head's sum of squares is a shuffle over the group.  Heads
+// [0, H) are scaled by w_q, [H, H + KVH) by w_k; the V heads are not touched.  Item `it` = row * (H + KVH) + head, so
+// rstd[it] and the pre-norm copy xqk[it * hd ...] ([M, (H + KVH) * hd], what the backward rebuilds xhat from) are
+// contiguous per row.  fp32 math, one rounding to bf16.
+template <int HD>
+B200_DEVINL unsigned qk_group_mask() {
+  constexpr int G = HD / 8;
+  return (G == 32 ? 0xffffffffu : ((1u << G) - 1u) << ((threadIdx.x & 31) & ~(G - 1)));
+}
+
+template <int HD>
+__global__ void __launch_bounds__(256) qk_norm_rope_kernel(__nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ xqk,
+                                                           float* __restrict__ rstd, const __nv_bfloat16* __restrict__ wq,
+                                                           const __nv_bfloat16* __restrict__ wk,
+                                                           const float* __restrict__ table, int M, int seq_len,
+                                                           int row_stride, int H, int nh, float eps) {
+  constexpr int G = HD / 8;
+  const int lane = threadIdx.x % G;
+  const unsigned mask = qk_group_mask<HD>();
+  float wqv[8], wkv[8];
+  load8(wq + lane * 8, wqv);
+  load8(wk + lane * 8, wkv);
+  const size_t items = (size_t)M * nh, step = (size_t)gridDim.x * (blockDim.x / G);
+  for (size_t it = (size_t)blockIdx.x * (blockDim.x / G) + threadIdx.x / G; it < items; it += step) {
+    const size_t row = it / nh;
+    const int head = (int)(it - row * nh);
+    __nv_bfloat16* p = qkv + row * row_stride + head * HD + lane * 8;
+    const uint4 raw = *reinterpret_cast<const uint4*>(p);
+    const float* trow = table + (size_t)(row % seq_len) * HD + lane * 8;   // [hd/2][cos, sin], this lane's 4 pairs
+    const float4 c0 = reinterpret_cast<const float4*>(trow)[0], c1 = reinterpret_cast<const float4*>(trow)[1];
+    float x[8];
+    unpack8(raw, x);
+    float ss = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) ss += x[i] * x[i];
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) ss += __shfl_xor_sync(mask, ss, o);
+    const float r = rsqrtf(ss / (float)HD + eps);
+    const bool isq = head < H;
+    float y[8], out[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) y[i] = x[i] * r * (isq ? wqv[i] : wkv[i]);
+    const float cosv[4] = {c0.x, c0.z, c1.x, c1.z}, sinv[4] = {c0.y, c0.w, c1.y, c1.w};
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      out[2 * i] = y[2 * i] * cosv[i] - y[2 * i + 1] * sinv[i];
+      out[2 * i + 1] = y[2 * i] * sinv[i] + y[2 * i + 1] * cosv[i];
+    }
+    store8(p, out);
+    *reinterpret_cast<uint4*>(xqk + it * HD + lane * 8) = raw;
+    if (lane == 0) rstd[it] = r;
+  }
+}
+
+// Backward of the norm, in place on the q / k sections of dqkv, which hold g = dL/d(xhat * w) (the attention backward
+// already applied the inverse RoPE): dx = rstd * (w * g - xhat * mean(xhat * w * g)).  dw = sum g * xhat over the rows
+// of the q heads (w_q) and of the k heads (w_k): every thread keeps its 8 columns for both, the CTA folds its groups in
+// a fixed order into dw_part[cta][2][hd], and colsum_kernel sums the CTAs in a fixed order -- no float atomics, so two
+// runs give the same bits.
+template <int HD>
+__global__ void __launch_bounds__(256) qk_norm_bwd_kernel(__nv_bfloat16* __restrict__ dqkv, const __nv_bfloat16* __restrict__ xqk,
+                                                          const float* __restrict__ rstd, const __nv_bfloat16* __restrict__ wq,
+                                                          const __nv_bfloat16* __restrict__ wk, float* __restrict__ dw_part,
+                                                          int M, int row_stride, int H, int nh) {
+  constexpr int G = HD / 8, NG = 256 / G;
+  __shared__ float sh[NG][2 * HD];
+  const int lane = threadIdx.x % G, grp = threadIdx.x / G;
+  const unsigned mask = qk_group_mask<HD>();
+  float wqv[8], wkv[8], accq[8], acck[8];
+  load8(wq + lane * 8, wqv);
+  load8(wk + lane * 8, wkv);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) accq[i] = acck[i] = 0.f;
+  const size_t items = (size_t)M * nh, step = (size_t)gridDim.x * NG;
+  for (size_t it = (size_t)blockIdx.x * NG + grp; it < items; it += step) {
+    const size_t row = it / nh;
+    const int head = (int)(it - row * nh);
+    __nv_bfloat16* p = dqkv + row * row_stride + head * HD + lane * 8;
+    float g[8], x[8];
+    load8(p, g);
+    load8(xqk + it * HD + lane * 8, x);
+    const float r = rstd[it];
+    const bool isq = head < H;
+    float dot = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      x[i] *= r;                                             // xhat
+      const float gx = g[i] * x[i];
+      dot += gx * (isq ? wqv[i] : wkv[i]);
+      accq[i] += isq ? gx : 0.f;
+      acck[i] += isq ? 0.f : gx;
+    }
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) dot += __shfl_xor_sync(mask, dot, o);
+    dot /= (float)HD;
+    float out[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) out[i] = r * ((isq ? wqv[i] : wkv[i]) * g[i] - x[i] * dot);
+    store8(p, out);
+  }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    sh[grp][lane * 8 + i] = accq[i];
+    sh[grp][HD + lane * 8 + i] = acck[i];
+  }
+  __syncthreads();
+  for (int c = threadIdx.x; c < 2 * HD; c += blockDim.x) {
+    float s = 0.f;
+#pragma unroll 8
+    for (int k = 0; k < NG; ++k) s += sh[k][c];
+    dw_part[(size_t)blockIdx.x * 2 * HD + c] = s;
+  }
+}
+
 static inline int grid_for(size_t work_items, int threads, int max_blocks = 132 * 8) {
   size_t b = (work_items + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -884,6 +1001,35 @@ extern "C" int b200_sumsq(const void* x, int is_bf16, long long n, float* out, c
   int g = grid_for((size_t)n / 16, 256, 132 * 8);
   if (is_bf16) sumsq_kernel<__nv_bfloat16><<<g, 256, 0, s>>>((const __nv_bfloat16*)x, (size_t)n, out);
   else sumsq_kernel<float><<<g, 256, 0, s>>>((const float*)x, (size_t)n, out);
+  CK();
+}
+extern "C" int b200_qk_norm_rope(void* qkv, void* xqk, float* rstd, const void* wq, const void* wk, const float* table,
+                                 int M, int seq_len, int row_stride, int H, int KVH, int hd, float eps, cudaStream_t s) {
+  if ((hd != 64 && hd != 128) || row_stride % 8 || M <= 0) return -1;
+  const size_t threads = (size_t)M * (H + KVH) * (hd / 8);
+#define B200_QKN_FWD(HDV)                                                                                         \
+  qk_norm_rope_kernel<HDV><<<grid_for(threads, 256, 132 * 16), 256, 0, s>>>(                                      \
+      (__nv_bfloat16*)qkv, (__nv_bfloat16*)xqk, rstd, (const __nv_bfloat16*)wq, (const __nv_bfloat16*)wk, table, M, \
+      seq_len, row_stride, H, H + KVH, eps)
+  if (hd == 64) B200_QKN_FWD(64); else B200_QKN_FWD(128);
+#undef B200_QKN_FWD
+  CK();
+}
+// fixed for a given shape (the reduction order, and so the bits, depend on it)
+extern "C" int b200_qk_norm_bwd_grid(int M, int nh, int hd) {
+  return grid_for((size_t)M * nh * (hd / 8), 256, 132 * 4);
+}
+extern "C" int b200_qk_norm_bwd(void* dqkv, const void* xqk, const float* rstd, const void* wq, const void* wk,
+                                float* dw_part, float* dw, int M, int row_stride, int H, int KVH, int hd, cudaStream_t s) {
+  if ((hd != 64 && hd != 128) || row_stride % 8 || M <= 0) return -1;
+  const int grid = b200_qk_norm_bwd_grid(M, H + KVH, hd);
+#define B200_QKN_BWD(HDV)                                                                                         \
+  qk_norm_bwd_kernel<HDV><<<grid, 256, 0, s>>>((__nv_bfloat16*)dqkv, (const __nv_bfloat16*)xqk, rstd,              \
+                                               (const __nv_bfloat16*)wq, (const __nv_bfloat16*)wk, dw_part, M,     \
+                                               row_stride, H, H + KVH)
+  if (hd == 64) B200_QKN_BWD(64); else B200_QKN_BWD(128);
+#undef B200_QKN_BWD
+  colsum_kernel<<<(2 * hd + 31) / 32, 256, 0, s>>>(dw_part, dw, grid, 2 * hd);
   CK();
 }
 

@@ -4,6 +4,8 @@ the adapters of ``train_speculator_utils.py:526-569``):
 
 * Llama   -> ``LLaMA`` / ``EmbedLLaMA``: fuses q/k/v and gate/up, permutes q/k rows from HF's half-split RoPE layout back
   to the FMS interleaved-pair layout (the inverse of ``fms_to_hf_llama._interleaved_to_halfsplit``);
+* Qwen3 (dense) -> ``LLaMA`` with ``qk_norm`` and an explicit head dim: as Llama, plus the per-head ``q_norm`` / ``k_norm``
+  gains permuted the same way as the q / k rows (tied embeddings are read as an untied copy);
 * GPT-BigCode (multi-query attention, learned positions) -> ``EmbedGPTBigCode``;
 * Mixtral (Llama attention + top-k sparse MoE) -> ``EmbedMixtral``; both the hub format (``block_sparse_moe.experts.N.w1/w2/w3``)
   and the fused in-memory format of recent transformers (``mlp.experts.gate_up_proj / down_proj``)."""
@@ -12,7 +14,7 @@ from __future__ import annotations
 import glob
 import json
 import os
-from typing import Dict
+from typing import Dict, Optional
 
 import torch
 
@@ -23,15 +25,34 @@ def _halfsplit_to_interleaved(w: torch.Tensor, nheads: int) -> torch.Tensor:
     return w.view(nheads, 2, -1, w.size(1)).transpose(1, 2).reshape(*w.size())
 
 
+def _halfsplit_to_interleaved_vec(w: torch.Tensor) -> torch.Tensor:
+    """A per-head-position vector [hd] (Qwen3 ``q_norm`` / ``k_norm``) in the order of the permuted q / k rows:
+    out[2i] = w[i], out[2i + 1] = w[i + hd/2].  RMS is permutation-invariant, the elementwise gain is not."""
+    return _halfsplit_to_interleaved(w.view(-1, 1), 1).view(-1)
+
+
+# model types whose differences from the Llama block are not implemented here (loading them would change the logits)
+_REFUSED_MODEL_TYPES = {
+    "olmo2": "q / k RMSNorm over the whole projection instead of per head",
+    "olmo3": "q / k RMSNorm over the whole projection instead of per head",
+    "qwen2": "q / k / v projection biases",
+    "qwen3_moe": "sparse mixture-of-experts feed-forward",
+}
+
+
 def _refuse_unsupported(hf_cfg: dict):
     """Features this repo's models do not implement must stop the load instead of silently changing the logits."""
+    why = _REFUSED_MODEL_TYPES.get(hf_cfg.get("model_type"))
+    if why:
+        raise NotImplementedError(f"HF model type {hf_cfg['model_type']!r} is not supported ({why}); Llama and Qwen3 dense "
+                                  "checkpoints are")
     scaling = hf_cfg.get("rope_scaling") or {}
     params = hf_cfg.get("rope_parameters") or {}
     kind = scaling.get("rope_type") or scaling.get("type") or params.get("rope_type") or "default"
     if kind not in ("default", None, "llama3", "linear"):
         raise NotImplementedError(f"HF checkpoint uses rope scaling {kind!r}; plain RoPE, 'linear' and 'llama3' (Llama 3.1 / 3.2) "
                                   "are implemented, loading it would change the logits")
-    window = hf_cfg.get("sliding_window")
+    window = hf_cfg.get("sliding_window") if hf_cfg.get("use_sliding_window", True) else None
     if window and window < hf_cfg.get("max_position_embeddings", window):
         raise NotImplementedError(f"HF checkpoint uses sliding-window attention (window {window}); only full causal attention is "
                                   "implemented")
@@ -39,19 +60,32 @@ def _refuse_unsupported(hf_cfg: dict):
         raise NotImplementedError("HF checkpoint has attention / MLP biases; the LLaMA blocks here are bias-free")
 
 
-def config_from_hf(hf_cfg: dict) -> LLaMAConfig:
+_Q_NORM_KEY = "model.layers.0.self_attn.q_norm.weight"
+
+
+def config_from_hf(hf_cfg: dict, tensors: Optional[Dict[str, torch.Tensor]] = None) -> LLaMAConfig:
+    """``tensors`` (optional): the checkpoint's tensors; a per-head ``self_attn.q_norm.weight`` there turns QK-norm on
+    whatever ``model_type`` says."""
     _refuse_unsupported(hf_cfg)
     D, F = hf_cfg["hidden_size"], hf_cfg["intermediate_size"]
+    H = hf_cfg["num_attention_heads"]
+    hd = hf_cfg.get("head_dim") or D // H
+    qk_norm = hf_cfg.get("model_type") == "qwen3"
+    if tensors is not None and _Q_NORM_KEY in tensors:
+        if tensors[_Q_NORM_KEY].numel() != hd:
+            raise NotImplementedError(f"HF checkpoint normalises q over {tensors[_Q_NORM_KEY].numel()} features; only a "
+                                      f"per-head QK-norm (weight [head_dim = {hd}], Qwen3) is implemented")
+        qk_norm = True
     rope = hf_cfg.get("rope_theta") or (hf_cfg.get("rope_parameters") or {}).get("rope_theta", 10000.0)
     scaling = hf_cfg.get("rope_scaling") or hf_cfg.get("rope_parameters") or {}
     kind = scaling.get("rope_type") or scaling.get("type")
     rope_scaling = {k: v for k, v in scaling.items() if k != "rope_theta"} if kind in ("llama3", "linear") else None
     return LLaMAConfig(
         src_vocab_size=hf_cfg["vocab_size"], emb_dim=D, norm_eps=hf_cfg.get("rms_norm_eps", 1e-5),
-        nheads=hf_cfg["num_attention_heads"], kvheads=hf_cfg.get("num_key_value_heads", 0) or 0,
+        nheads=H, kvheads=hf_cfg.get("num_key_value_heads", 0) or 0,
         nlayers=hf_cfg["num_hidden_layers"], hidden_grow_factor=F / D, multiple_of=1,
         max_expected_seq_len=hf_cfg.get("max_position_embeddings", 4096), rope_theta=float(rope),
-        rope_scaling=rope_scaling)
+        rope_scaling=rope_scaling, qk_norm=qk_norm, attn_head_dim=hd if hd != D // H else None)
 
 
 def _read_hf_tensors(model_path: str) -> Dict[str, torch.Tensor]:
@@ -83,16 +117,27 @@ def convert_hf_state_dict(hf: Dict[str, torch.Tensor], cfg: LLaMAConfig) -> Dict
         sd[d + "ff_sub_layer.w2.weight"] = hf[s + "mlp.down_proj.weight"]
         sd[d + "ln.weight"] = hf[s + "input_layernorm.weight"]
         sd[d + "ff_ln.weight"] = hf[s + "post_attention_layernorm.weight"]
+        if (s + "self_attn.q_norm.weight" in hf) != bool(cfg.qk_norm):
+            raise ValueError(f"layer {i}: the checkpoint {'lacks' if cfg.qk_norm else 'has'} q / k norm weights "
+                             f"but the config says qk_norm={cfg.qk_norm}")
+        if cfg.qk_norm:   # per-head gains follow the q / k rows from half-split to interleaved order
+            for name in ("q_norm", "k_norm"):
+                w = hf[s + f"self_attn.{name}.weight"]
+                if w.numel() != cfg.head_dim:
+                    raise NotImplementedError(f"{s}self_attn.{name}.weight has {w.numel()} elements; only a per-head "
+                                              f"QK-norm over head_dim = {cfg.head_dim} is implemented")
+                sd[d + f"attn.{name}.weight"] = _halfsplit_to_interleaved_vec(w)
     return sd
 
 
 def load_hf_llama(model_path: str, device="cpu", dtype=torch.bfloat16, model_cls=LLaMA) -> LLaMA:
+    tensors = _read_hf_tensors(model_path)
     with open(os.path.join(model_path, "config.json")) as f:
-        cfg = config_from_hf(json.load(f))
+        cfg = config_from_hf(json.load(f), tensors)
     with torch.device("meta"):
         model = model_cls(cfg)
     model.to_empty(device=device)
-    sd = convert_hf_state_dict(_read_hf_tensors(model_path), cfg)
+    sd = convert_hf_state_dict(tensors, cfg)
     model.load_state_dict({k: v.to(dtype) for k, v in sd.items()})
     return model.to(dtype)
 

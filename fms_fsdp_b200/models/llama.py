@@ -51,6 +51,12 @@ class LLaMAConfig:
     # attention is masked at document boundaries.  RoPE positions stay absolute: rotary scores depend only on position
     # differences, so a document in the middle of a row attends exactly as it would from position 0.
     doc_separator: Optional[int] = None
+    # extension (not an fms field): QK-norm (Qwen3) -- a per-head RMSNorm of q and k (weights ``attn.q_norm`` /
+    # ``attn.k_norm`` [head_dim], eps ``norm_eps``) after the projection and before RoPE.
+    qk_norm: bool = False
+    # extension (not an fms field): head dimension when it is not emb_dim // nheads (Qwen3-0.6B / 4B: 128 with
+    # emb_dim / nheads = 64 / 80).  None = emb_dim // nheads.
+    attn_head_dim: Optional[int] = None
 
     @property
     def hidden_dim(self) -> int:
@@ -63,7 +69,7 @@ class LLaMAConfig:
 
     @property
     def head_dim(self) -> int:
-        return self.emb_dim // self.nheads
+        return self.attn_head_dim if self.attn_head_dim else self.emb_dim // self.nheads
 
 
 class _Weight(nn.Module):
@@ -143,10 +149,21 @@ class MultiHeadAttention(nn.Module):
         self.emb_dim = cfg.emb_dim
         self.in_proj = _InProj(cfg, device, dtype)
         self.dense = _Weight(cfg.emb_dim, cfg.nheads * cfg.head_dim, device, dtype)
+        self.qk_norm = bool(cfg.qk_norm)
+        if self.qk_norm:   # per-head gains, indexed by position within a head (interleaved RoPE pair order)
+            self.q_norm = RMSNorm(cfg.head_dim, cfg.norm_eps, device, dtype)
+            self.k_norm = RMSNorm(cfg.head_dim, cfg.norm_eps, device, dtype)
 
     def reset_parameters(self):
         for w in (self.in_proj.qkv_fused.weight, self.dense.weight):
             nn.init.trunc_normal_(w, mean=0.0, std=0.02)
+        if self.qk_norm:
+            self.q_norm.reset_parameters()
+            self.k_norm.reset_parameters()
+
+    def qk_norm_args(self):
+        """``ops.qkv_attention(qk_norm=...)``: None without QK-norm."""
+        return (self.q_norm.weight, self.k_norm.weight, self.q_norm.eps) if self.qk_norm else None
 
 
 class GatedLinearUnit(nn.Module):
@@ -208,7 +225,7 @@ class LLaMABlock(nn.Module):
         h, x = self.ln.fork(x)
         # projection + RoPE + attention: one node, RoPE fused into the GEMM / dq-dk epilogues
         ctx = ops.qkv_attention(h, a.in_proj.qkv_fused.weight, self._rot.table(x.device, S), a.nheads, a.kvheads,
-                                a.head_dim, doc=doc)
+                                a.head_dim, doc=doc, qk_norm=a.qk_norm_args())
         x = a.dense(ctx, residual=x)
         h, x = self.ff_ln.fork(x)
         ff = self.ff_sub_layer

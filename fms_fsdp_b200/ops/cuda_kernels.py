@@ -353,6 +353,30 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, inverse=
     return qkv
 
 
+# -------------------------------------------------------------------------------------- QK-norm
+def _qk_norm_native(t, head_dim, nheads, kvheads):
+    return (t.dtype == torch.bfloat16 and head_dim in (64, 128) and t.dim() == 2 and t.stride(-1) == 1
+            and t.stride(0) % 8 == 0 and t.data_ptr() % 16 == 0 and kvheads > 0 and nheads % kvheads == 0)
+
+
+def qk_norm_rope(qkv, w_q, w_k, table, seq_len, nheads, kvheads, head_dim, eps):
+    """Per-head RMSNorm (weights ``w_q`` / ``w_k`` [hd]) then interleaved RoPE of the q and k heads of ``qkv``
+    [M, (H + 2 KVH) * hd], in place; returns (pre-norm q / k [M, (H + KVH) * hd], rstd [M, H + KVH] fp32)."""
+    if not _qk_norm_native(qkv, head_dim, nheads, kvheads):
+        return _fallback("qk_norm_rope").qk_norm_rope(qkv, w_q, w_k, table, seq_len, nheads, kvheads, head_dim, eps)
+    xqk, rstd = _C.qk_norm_rope(qkv, _bf16c(w_q), _bf16c(w_k), table, int(seq_len), nheads, kvheads, head_dim, float(eps))
+    return xqk, rstd
+
+
+def qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim):
+    """In place on the q / k heads of ``dqkv`` (the gradient of the normed, un-rotated heads); returns fp32 (dw_q, dw_k),
+    reduced in a fixed order (bitwise reproducible)."""
+    if not (_qk_norm_native(dqkv, head_dim, nheads, kvheads) and xqk.dtype == torch.bfloat16 and xqk.is_contiguous()):
+        return _fallback("qk_norm_bwd").qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim)
+    dw_q, dw_k = _C.qk_norm_bwd(dqkv, xqk, rstd.contiguous(), _bf16c(w_q), _bf16c(w_k), nheads, kvheads, head_dim)
+    return dw_q, dw_k
+
+
 # ------------------------------------------------------------------------------------- attention
 def _sdpa_fwd(qkv, B, S, H, KVH, hd, scale, seg=None):
     q, k, v = torch_kernels._split_qkv(qkv, B, S, H, KVH, hd)

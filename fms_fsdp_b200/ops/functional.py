@@ -335,11 +335,91 @@ class _QKVAttention(torch.autograd.Function):
         return dh, dw, None, None, None, None, None, None, None
 
 
-def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None):
+def _put_fp32(val):
+    def put(out, acc):
+        if acc:
+            out.add_(val.to(out.dtype))
+        else:
+            out.copy_(val)
+    return put
+
+
+class _QKNormAttention(torch.autograd.Function):
+    """QKV projection + per-head QK RMSNorm + RoPE + causal attention as ONE autograd node.  Forward: plain QKV GEMM,
+    ``qk_norm_rope`` in place on the q / k heads (it keeps the pre-norm q / k and rstd for the backward), attention.
+    Backward: attention backward with the inverse RoPE fused into its dq / dk epilogues, ``qk_norm_bwd`` in place, then
+    the dgrad / wgrad GEMMs; the two norm vectors' gradients go through the runtime's buffers like ``ln`` / ``ff_ln``."""
+
+    @staticmethod
+    def forward(ctx, h, w, w_q, w_k, table, S, H, KVH, hd, scale, seg, eps):
+        K = kernels_for(h)
+        B = h.shape[0]
+        h2 = h.reshape(-1, h.shape[-1])
+        qkv = K.gemm(h2, _wdata(w), "nt")
+        xqk, rstd = K.qk_norm_rope(qkv, _wdata(w_q), _wdata(w_k), table, S, H, KVH, hd, eps)
+        o, lse = K.attn_fwd(qkv, B, S, H, KVH, hd, scale, seg=seg)
+        ctx.K, ctx.w, ctx.wqk, ctx.args, ctx.seg = K, w, (w_q, w_k), (B, S, H, KVH, hd, scale), seg
+        ctx.save_for_backward(h, qkv, o, lse, table, xqk, rstd)
+        return o.view(B, S, H * hd)
+
+    @staticmethod
+    def backward(ctx, do):
+        h, qkv, o, lse, table, xqk, rstd = ctx.saved_tensors
+        B, S, H, KVH, hd, scale = ctx.args
+        K, w, (w_q, w_k) = ctx.K, ctx.w, ctx.wqk
+        dqkv = K.attn_bwd(do.reshape(B * S, H * hd).contiguous(), qkv, o, lse, B, S, H, KVH, hd, scale,
+                          rope_table=table, seg=ctx.seg)
+        dwq32, dwk32 = K.qk_norm_bwd(dqkv, xqk, rstd, _wdata(w_q), _wdata(w_k), H, KVH, hd)
+        h2 = h.reshape(-1, h.shape[-1])
+        dh = K.gemm(dqkv, _wdata(w), "nn").view_as(h) if ctx.needs_input_grad[0] else None
+        dw = None
+        if ctx.needs_input_grad[1]:
+            dw = _deliver_wgrad(w, lambda out, acc: K.gemm(dqkv, h2, "tn", out=out, accumulate=acc))
+        dwq = _deliver_wgrad(w_q, _put_fp32(dwq32)) if ctx.needs_input_grad[2] else None
+        dwk = _deliver_wgrad(w_k, _put_fp32(dwk32)) if ctx.needs_input_grad[3] else None
+        return dh, dw, dwq, dwk, None, None, None, None, None, None, None, None
+
+
+class _QKNormRope(torch.autograd.Function):
+    """Stand-alone QK-norm + RoPE in place on a fused projection (the fp8 branch, whose projection is a separate GEMM)."""
+
+    @staticmethod
+    def forward(ctx, qkv, w_q, w_k, table, S, H, KVH, hd, eps):
+        K = kernels_for(qkv)
+        q2 = qkv.view(-1, qkv.shape[-1])
+        xqk, rstd = K.qk_norm_rope(q2, _wdata(w_q), _wdata(w_k), table, S, H, KVH, hd, eps)
+        ctx.K, ctx.wqk, ctx.args = K, (w_q, w_k), (S, H, KVH, hd)
+        ctx.save_for_backward(table, xqk, rstd)
+        ctx.mark_dirty(qkv)
+        return qkv
+
+    @staticmethod
+    def backward(ctx, dqkv):
+        table, xqk, rstd = ctx.saved_tensors
+        S, H, KVH, hd = ctx.args
+        w_q, w_k = ctx.wqk
+        # the normed projection feeds exactly one consumer (attention): its gradient is ours to rewrite in place
+        d = dqkv.contiguous()
+        d2 = d.view(-1, d.shape[-1])
+        ctx.K.rope_(d2, table, S, H, KVH, hd, hd, True, 0, True)
+        dwq32, dwk32 = ctx.K.qk_norm_bwd(d2, xqk, rstd, _wdata(w_q), _wdata(w_k), H, KVH, hd)
+        dwq = _deliver_wgrad(w_q, _put_fp32(dwq32)) if ctx.needs_input_grad[1] else None
+        dwk = _deliver_wgrad(w_k, _put_fp32(dwk32)) if ctx.needs_input_grad[2] else None
+        return d, dwq, dwk, None, None, None, None, None, None
+
+
+def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None, qk_norm=None):
     """attention(rope(h @ w^T)) for a fused [(H + 2 KVH) * hd, D] projection weight; h: [B, S, D].  ``doc``: the
-    ``document_segments`` table of a packed batch (attention stays inside each document), None = causal."""
+    ``document_segments`` table of a packed batch (attention stays inside each document), None = causal.
+    ``qk_norm=(w_q, w_k, eps)``: per-head RMSNorm of q and k (weights [hd]) between the projection and RoPE (Qwen3)."""
     S = h.shape[1]
     scale = (head_dim ** -0.5) if scale is None else scale
+    if qk_norm is not None:
+        w_q, w_k, eps = qk_norm
+        if _GEMM_PRECISION == "fp8":     # fp8 projection, then the stand-alone QK-norm + RoPE kernel and attention
+            qkv = _QKNormRope.apply(linear(h, w), w_q, w_k, table, S, nheads, kvheads, head_dim, eps)
+            return attention(qkv, nheads, kvheads, head_dim, scale, doc=doc)
+        return _QKNormAttention.apply(h, w, w_q, w_k, table, S, nheads, kvheads, head_dim, scale, doc, eps)
     if _GEMM_PRECISION == "fp8":     # fp8 projection, then the stand-alone RoPE kernel and attention
         return attention(rope_(linear(h, w), table, S, nheads, kvheads, head_dim), nheads, kvheads, head_dim, scale,
                          doc=doc)

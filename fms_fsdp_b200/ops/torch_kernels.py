@@ -156,6 +156,50 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, inverse=
 
 
 # ----------------------------------------------------------------------------------------------
+# QK-norm (Qwen3): per-head RMSNorm of the q and k heads with weights w_q / w_k [hd], then the interleaved RoPE, in place
+# on a fused [M, (H+2*KVH)*hd] projection.  The forward returns the pre-norm q / k [M, (H+KVH)*hd] and rstd [M, H+KVH]
+# (fp32); the backward takes the gradient of the normed, UN-rotated heads (the attention backward applies the inverse
+# RoPE) and returns fp32 (dw_q, dw_k).
+# ----------------------------------------------------------------------------------------------
+def _f32(t):
+    """fp32 math (fp64 inputs stay fp64, so the oracle itself can be checked in double precision)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
+def _qk_weights(w_q, w_k, nheads, kvheads):
+    return torch.cat([_f32(w_q).expand(nheads, -1), _f32(w_k).expand(kvheads, -1)])   # [H+KVH, hd]
+
+
+def qk_norm_rope(qkv, w_q, w_k, table, seq_len, nheads, kvheads, head_dim, eps):
+    M, nh = qkv.shape[0], nheads + kvheads
+    v = qkv.view(M, nheads + 2 * kvheads, head_dim)[:, :nh]
+    xqk = v.reshape(M, nh * head_dim).clone()
+    x = _f32(v)
+    rstd = torch.rsqrt(x.pow(2).mean(-1) + eps)
+    y = (x * rstd.unsqueeze(-1) * _qk_weights(w_q, w_k, nheads, kvheads)).reshape(M, nh * head_dim)
+    cs = table[torch.arange(M, device=qkv.device) % seq_len]                      # [M, hd/2, 2]
+    cos, sin = cs[..., 0].unsqueeze(1), cs[..., 1].unsqueeze(1)
+    y = y.view(M, nh, head_dim // 2, 2)
+    y0, y1 = y[..., 0], y[..., 1]
+    v.copy_(torch.stack([y0 * cos - y1 * sin, y0 * sin + y1 * cos], dim=-1).reshape(M, nh, head_dim).to(qkv.dtype))
+    return xqk, rstd
+
+
+def qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim):
+    M, nh = dqkv.shape[0], nheads + kvheads
+    gv = dqkv.view(M, nheads + 2 * kvheads, head_dim)[:, :nh]
+    g = _f32(gv)
+    r = _f32(rstd.view(M, nh, 1))
+    xhat = _f32(xqk.view(M, nh, head_dim)) * r
+    w = _qk_weights(w_q, w_k, nheads, kvheads)
+    dx = r * (w * g - xhat * (g * w * xhat).mean(-1, keepdim=True))
+    gx = g * xhat
+    dw_q, dw_k = gx[:, :nheads].sum((0, 1)), gx[:, nheads:].sum((0, 1))
+    gv.copy_(dx.to(dqkv.dtype))
+    return dw_q, dw_k
+
+
+# ----------------------------------------------------------------------------------------------
 # Causal flash attention on the fused projection.  qkv: [B*S, (H+2KVH)*hd]; o: [B*S, H*hd];
 # lse: [B, H, S] fp32 (natural log).
 # ----------------------------------------------------------------------------------------------

@@ -33,6 +33,15 @@ def _slice_llama_attention(blk, c, tp: int, r: int):
     blk.attn.nheads, blk.attn.kvheads = H, KV
 
 
+def refuse_unsupported_base(c):
+    """The frozen-base attention of speculator training (``EmbedLLaMA``, the TP slicing here) projects, rotates and
+    attends on its own; it has no QK-norm and assumes head_dim = emb_dim / nheads.  Running such a base without its
+    norms would give wrong hidden states, so it is refused."""
+    if getattr(c, "qk_norm", False) or getattr(c, "attn_head_dim", None) not in (None, c.emb_dim // c.nheads):
+        raise NotImplementedError("speculator base models with QK-norm or a head_dim other than emb_dim / nheads "
+                                  "(e.g. Qwen3) are not supported: the frozen-base attention path has no QK-norm")
+
+
 def _check_llama_divisible(c, tp: int):
     assert c.nheads % tp == 0 and c.kv_heads % tp == 0 and c.hidden_dim % tp == 0 and c.src_vocab_size % tp == 0, \
         "tp size must divide heads, kv heads, hidden dim and vocab"
@@ -43,6 +52,7 @@ def shard_llama_for_tp(model: LLaMA, group) -> LLaMA:
     of the MLP hidden units.  The model is flagged so ``EmbedLLaMA.forward`` inserts the collectives."""
     tp, r = dist.get_world_size(group), dist.get_rank(group)
     c = model.config
+    refuse_unsupported_base(c)
     _check_llama_divisible(c, tp)
     F = c.hidden_dim // tp
     with torch.no_grad():
@@ -62,6 +72,7 @@ def shard_mixtral_for_tp(model, group):
     all-reduced like a row-parallel linear."""
     tp, r = dist.get_world_size(group), dist.get_rank(group)
     c = model.config
+    refuse_unsupported_base(c)
     _check_llama_divisible(c, tp)
     F = c.hidden_dim // tp
     with torch.no_grad():

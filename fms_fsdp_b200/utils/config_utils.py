@@ -42,6 +42,14 @@ def _llama3(emb_dim, nheads, nlayers, grow, seq):
                 hidden_grow_factor=grow, max_expected_seq_len=seq, rope_theta=500000.0)
 
 
+def _qwen3(emb_dim, ffn, nlayers, nheads):
+    """Qwen3 dense: the Llama block with QK-norm and head_dim 128 (not always emb_dim / nheads).  multiple_of=1 and
+    grow = ffn / emb_dim give hidden_dim == ffn exactly, as ``models/hf_loader.config_from_hf`` builds it."""
+    return dict(src_vocab_size=151936, emb_dim=emb_dim, nheads=nheads, kvheads=8, nlayers=nlayers,
+                hidden_grow_factor=ffn / emb_dim, multiple_of=1, max_expected_seq_len=40960, rope_theta=1000000.0,
+                norm_eps=1e-6, qk_norm=True, attn_head_dim=128)
+
+
 _LLAMA_ZOO: Dict[str, Dict[str, Any]] = {
     "llama2_70b": dict(emb_dim=8192, multiple_of=4096, nheads=64, kvheads=8, nlayers=80,
                        hidden_grow_factor=28672 / 8192),
@@ -63,6 +71,11 @@ _LLAMA_ZOO: Dict[str, Dict[str, Any]] = {
     # --- extensions (BASELINE.json config #1; plumbing / CPU-gloo tests)
     "llama2_tiny": dict(src_vocab_size=1024, emb_dim=256, nheads=4, kvheads=4, nlayers=2,
                         hidden_grow_factor=8 / 3, multiple_of=64, max_expected_seq_len=512),
+    # --- extensions: Qwen3 dense checkpoints (hf_to_fms_llama.py imports them; the tied 0.6B / 1.7B / 4B heads untied)
+    "qwen3_0.6b": _qwen3(1024, 3072, 28, 16),
+    "qwen3_1.7b": _qwen3(2048, 6144, 28, 16),
+    "qwen3_4b": _qwen3(2560, 9728, 36, 32),
+    "qwen3_8b": _qwen3(4096, 12288, 36, 32),
 }
 
 _MAMBA_ZOO: Dict[str, Dict[str, Any]] = {

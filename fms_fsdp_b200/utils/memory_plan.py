@@ -13,8 +13,9 @@ The numbers follow what the runtime allocates (``parallel/engine.py``) and what 
 * gradient staging (sharded only): ``push_pool`` block-sized buffers the wgrad GEMMs of all ranks push into, plus the root
   unit's unsharded gradient (pull path);
 * activations per block kept for backward (bf16; T = batch * seq tokens): block input, two normed inputs, rotated QKV,
-  attention output, post-attention residual, gate|up and SwiGLU output = 2T(6D + 2*KV*hd + 3F) bytes, plus fp32 row
-  statistics; a recomputed block keeps its input only, one block's worth of activations is live while it is recomputed;
+  attention output, post-attention residual, gate|up and SwiGLU output = 2T(4D + 2*H*hd + 2*KV*hd + 3F) bytes, plus fp32
+  row statistics; with QK-norm also the pre-norm q / k, 2T(H + KV)*hd bytes, and their rstd, 4T(H + KV) bytes; a
+  recomputed block keeps its input only, one block's worth of activations is live while it is recomputed;
 * head: the final hidden states, their gradient and one [4096, V] logits chunk (+ its gradient in place).
 
 Checked against the measured peak of the caching allocator: Llama2-1.4B, 1 H100 80GB HBM3 (400 W limit), seq 4096,
@@ -75,7 +76,9 @@ def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp
     S = resolve_shard_size(sharding_strategy, gpus, hsdp_shard_size, None)
     T = batch_size * seq_length
 
-    block_params = (c.nheads * hd + 2 * kvd) * D + D * c.nheads * hd + 2 * F * D + D * F + 2 * D
+    qd = c.nheads * hd
+    qk_norm = bool(getattr(c, "qk_norm", False))
+    block_params = (qd + 2 * kvd) * D + D * qd + 2 * F * D + D * F + 2 * D + (2 * hd if qk_norm else 0)
     root_params = 2 * V * D + D
     n_params = L * block_params + root_params
 
@@ -89,7 +92,9 @@ def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp
         parts[f"gathered parameters ({prefetch + 1} blocks + root, bf16)"] = 2.0 * ((prefetch + 1) * block_params + root_params) / GiB
         parts[f"gradient staging ({push_pool} block buffers + root, bf16)"] = 2.0 * (push_pool * block_params + root_params) / GiB
 
-    per_block = 2.0 * T * (6 * D + 2 * kvd + 3 * F) + 4.0 * T * (2 + c.nheads)    # bf16 tensors + rstd x2 + lse
+    per_block = 2.0 * T * (4 * D + 2 * qd + 2 * kvd + 3 * F) + 4.0 * T * (2 + c.nheads)    # bf16 tensors + rstd x2 + lse
+    if qk_norm:   # the QK-norm node also keeps the pre-norm q / k (bf16) and their per-head rstd (fp32)
+        per_block += 2.0 * T * (qd + kvd) + 4.0 * T * (c.nheads + c.kv_heads)
     n_re = _recomputed_blocks(L, selective_checkpointing, fsdp_activation_checkpointing)
     kept = (L - n_re) * per_block + n_re * 2.0 * T * D + (per_block if n_re else 0.0)
     parts[f"activations ({L - n_re} blocks kept, {n_re} recomputed)"] = kept / GiB

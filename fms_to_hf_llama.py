@@ -1,4 +1,5 @@
-"""Export a sharded training checkpoint to a HuggingFace ``LlamaForCausalLM`` directory
+"""Export a sharded training checkpoint to a HuggingFace ``LlamaForCausalLM`` directory (``Qwen3ForCausalLM`` for variants
+with QK-norm)
 (CLI parity with reference ``fms_to_hf_llama.py:133-171``):
 
     python fms_to_hf_llama.py --model_variant llama2_7b --nocompiled --load_path <step_N_ckp> \
@@ -24,9 +25,15 @@ def _interleaved_to_halfsplit(w: torch.Tensor, nheads: int) -> torch.Tensor:
     return w.view(nheads, -1, 2, w.size(1)).transpose(1, 2).reshape(*w.size())
 
 
+def _interleaved_to_halfsplit_vec(w: torch.Tensor) -> torch.Tensor:
+    """Per-head-position gains [hd] (``q_norm`` / ``k_norm``) in HF's half-split order: out[i] = w[2i], out[i + hd/2] = w[2i + 1]."""
+    return _interleaved_to_halfsplit(w.view(-1, 1), 1).view(-1)
+
+
 def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
     """``is_old_fms`` is kept for the reference's signature; this repo's LLaMA is always fused, pre-fusion checkpoints are
-    fused when they are read (``load_dcp_into``)."""
+    fused when they are read (``load_dcp_into``).  A model with ``qk_norm`` is written as a ``Qwen3ForCausalLM`` (untied
+    head), every other one as a ``LlamaForCausalLM``."""
     from transformers import LlamaConfig, LlamaForCausalLM
 
     c = model.config
@@ -44,7 +51,15 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
         kw.update(bos_token_id=128000, eos_token_id=128001)
     if getattr(c, "rope_scaling", None):          # long-context frequency rescaling travels with the export
         kw["rope_scaling"] = dict(c.rope_scaling)
-    hf = LlamaForCausalLM(LlamaConfig(**kw))
+    if getattr(c, "attn_head_dim", None):
+        kw["head_dim"] = c.head_dim
+    if getattr(c, "qk_norm", False):
+        from transformers import Qwen3Config, Qwen3ForCausalLM
+        kw.pop("mlp_bias")
+        kw["head_dim"] = c.head_dim
+        hf = Qwen3ForCausalLM(Qwen3Config(**kw, use_sliding_window=False))
+    else:
+        hf = LlamaForCausalLM(LlamaConfig(**kw))
     sd = model.state_dict()
     hd = c.head_dim
     with torch.no_grad():
@@ -57,6 +72,9 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
             layer.self_attn.k_proj.weight.copy_(_interleaved_to_halfsplit(k, c.kv_heads))
             layer.self_attn.v_proj.weight.copy_(v)
             layer.self_attn.o_proj.weight.copy_(sd[p + "attn.dense.weight"])
+            if getattr(c, "qk_norm", False):
+                layer.self_attn.q_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.q_norm.weight"]))
+                layer.self_attn.k_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.k_norm.weight"]))
             fused = sd[p + "ff_sub_layer.wg1_fused.weight"]
             wg, w1 = torch.split(fused, [fused.size(0) // 2, fused.size(0) // 2], dim=0)
             layer.mlp.gate_proj.weight.copy_(wg)

@@ -57,6 +57,9 @@ def main(**kwargs):
     if cfg.document_attention_mask:
         # packed lines hold several documents, each ended by the loader's eos_token: attend within a document only
         llama_config.doc_separator = cfg.eos_token
+    if cfg.qk_norm:
+        # per-head RMSNorm of q and k before RoPE (the qwen3_* variants have it already)
+        llama_config.qk_norm = True
     if cfg.low_cpu_fsdp or use_cuda:
         # one unit at a time is materialised directly on the device by the sharded runtime
         with torch.device("meta"):

@@ -29,6 +29,9 @@ def main(**kwargs):
         raise ValueError("--document_attention_mask is not supported for Mamba models: the SSD scan and the causal "
                          "conv1d carry state across document boundaries, so masking only the attention layers "
                          "would not isolate documents")
+    if cfg.qk_norm:
+        raise ValueError("--qk_norm is not supported for Mamba models: their attention layers have no q / k norm "
+                         "weights, and the option would silently change nothing")
 
     use_cuda = torch.cuda.is_available() and cfg.comm_backend != "gloo"
     if use_cuda:

@@ -15,7 +15,7 @@ import torch.nn.functional as F
 
 from fms_fsdp_b200 import ops
 from fms_fsdp_b200.models.llama import LLaMA, LLaMAConfig
-from fms_fsdp_b200.parallel.tensor_parallel import tp_all_gather_last, tp_all_reduce
+from fms_fsdp_b200.parallel.tensor_parallel import refuse_unsupported_base, tp_all_gather_last, tp_all_reduce
 
 
 # ---------------------------------------------------------------------------------- base models
@@ -31,6 +31,10 @@ class EmbedLLaMA(LLaMA):
     Inference only: prefill uses the engine's flash attention; single-token decode steps attend over the
     cache with SDPA.  With ``shard_llama_for_tp`` applied, row-parallel outputs are all-reduced.
     Reference: ``speculator/train_speculator_utils.py:464-492``."""
+
+    def __init__(self, config: Optional[LLaMAConfig] = None, device=None, dtype=None, **kwargs):
+        super().__init__(config, device, dtype, **kwargs)
+        refuse_unsupported_base(self.config)
 
     def forward(self, x, mask=None, position_ids=None, past_key_value_states=None, use_cache=False,
                 only_last_token=False, attn_algorithm=None, include_embeds=False):
