@@ -110,3 +110,4 @@ class train_config:
     document_attention_mask: bool = False    # Llama: attention stops at eos_token in packed lines (RoPE positions are not reset)
     qk_norm: bool = False                    # Llama: per-head RMSNorm of q and k before RoPE (Qwen3 QK-norm), for any variant
     grad_accum_steps: int = 1                # micro-batches per optimizer step (global batch = world x batch_size x this)
+    moe_aux_loss_coef: Optional[float] = None  # MoE Llama: load-balancing loss coefficient (None = the variant's value)

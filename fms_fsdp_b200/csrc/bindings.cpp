@@ -80,6 +80,19 @@ DECL int b200_allreduce_inplace(void* const*, long long, int, int, int, float, f
 DECL int b200_signal_barrier(uint32_t* const*, int, int, uint32_t, int, int, cudaStream_t);
 DECL int b200_scalar_allreduce_bytes();
 DECL int b200_scalar_allreduce(uint8_t* const*, int, int, uint32_t, float*, int, cudaStream_t);
+DECL int b200_gemm_grouped_bf16(const void*, const void*, void*, const int*, const int*, int, int, int, int, int, int, int,
+                                int, int, int, int, cudaStream_t);
+DECL int b200_moe_route(const float*, int, int, int, int, float*, int*, float*, cudaStream_t);
+DECL int b200_moe_plan_ws_chunks(int);
+DECL int b200_moe_plan(const int*, const float*, int, int, int, int, int*, float*, int*, int*, int*, int*, int*, float*,
+                       cudaStream_t);
+DECL int b200_moe_permute(const void*, const int*, const int*, const int*, const int*, int, int, int, void*, cudaStream_t);
+DECL int b200_moe_permute_bwd(const void*, const int*, int, int, int, void*, cudaStream_t);
+DECL int b200_moe_combine(const void*, const int*, const float*, const void*, int, int, int, void*, cudaStream_t);
+DECL int b200_moe_combine_bwd(const void*, const void*, const float*, const int*, const int*, const int*, const int*, int,
+                              int, int, void*, float*, cudaStream_t);
+DECL int b200_moe_route_bwd(const float*, const int*, const float*, const float*, const int*, int, int, int, int, float,
+                            void*, cudaStream_t);
 DECL int b200_causal_conv1d_fwd(const void*, const void*, const void*, void*, int, int, int, int, int, cudaStream_t);
 DECL int b200_causal_conv1d_bwd(const void*, const void*, const void*, const void*, void*, float*, float*, int, int,
                                 int, int, int, cudaStream_t);
@@ -814,9 +827,185 @@ std::vector<at::Tensor> selective_scan_bwd(const at::Tensor& dy, const at::Tenso
   return {du, dd, dA, dB, dC, dD, dz, ddb};
 }
 
+// ---- mixture of experts (csrc/moe.cu).  The plan is one int32 buffer [tile NT | start E | len E | row T k | src Mpad]
+// with Mpad = round_up(T k + 127 E, 128) and NT = Mpad / 128 (ops/torch_kernels.py MoEPlan).
+struct MoEDims {
+  int T, k, E, Mpad, NT;
+  MoEDims(int64_t T_, int64_t k_, int64_t E_) : T((int)T_), k((int)k_), E((int)E_) {
+    Mpad = (int)((((int64_t)T * k + 127 * (int64_t)E) + 127) / 128 * 128);
+    NT = Mpad / 128;
+  }
+  int64_t numel() const { return (int64_t)NT + 2 * E + (int64_t)T * k + Mpad; }
+};
+struct PlanPtrs {
+  const int *tile, *start, *len, *row, *src;
+  PlanPtrs(const at::Tensor& plan, const MoEDims& d) {
+    need(plan, "plan", at::kInt);
+    TORCH_CHECK(plan.is_contiguous() && plan.numel() == d.numel(), "moe: plan has ", plan.numel(), " entries, expected ",
+                d.numel());
+    const int* p = plan.data_ptr<int>();
+    tile = p; start = p + d.NT; len = start + d.E; row = len + d.E; src = row + (int64_t)d.T * d.k;
+  }
+};
+inline void need_rows(const at::Tensor& t, const char* name, int64_t rows, int64_t cols) {
+  need(t, name, at::kBFloat16);
+  TORCH_CHECK(t.is_contiguous() && t.dim() == 2 && t.size(0) == rows && t.size(1) == cols && cols % 8 == 0, name,
+              " must be a contiguous [", rows, ", ", cols, "] bf16 tensor with a multiple of 8 columns");
+}
+
+std::vector<at::Tensor> moe_route(const at::Tensor& logits, int64_t k, bool norm) {
+  c10::cuda::CUDAGuard guard(logits.device());
+  need(logits, "logits", at::kFloat);
+  TORCH_CHECK(logits.dim() == 2 && logits.is_contiguous(), "moe_route: logits must be contiguous [T, E]");
+  const int T = logits.size(0), E = logits.size(1);
+  auto probs = at::empty({T, E}, logits.options());
+  auto ids = at::empty({T, k}, logits.options().dtype(at::kInt));
+  auto wts = at::empty({T, k}, logits.options());
+  check(b200_moe_route(logits.data_ptr<float>(), T, E, (int)k, norm ? 1 : 0, probs.data_ptr<float>(), ids.data_ptr<int>(),
+                       wts.data_ptr<float>(), cur_stream()), "moe_route");
+  return {ids, wts, probs};
+}
+
+std::vector<at::Tensor> moe_plan(const at::Tensor& ids, const at::Tensor& probs) {
+  c10::cuda::CUDAGuard guard(ids.device());
+  need(ids, "ids", at::kInt);
+  need(probs, "probs", at::kFloat);
+  TORCH_CHECK(ids.dim() == 2 && ids.is_contiguous() && probs.dim() == 2 && probs.is_contiguous() &&
+              probs.size(0) == ids.size(0), "moe_plan: ids [T, k] int32, probs [T, E] fp32");
+  const MoEDims d(ids.size(0), ids.size(1), probs.size(1));
+  auto plan = at::empty({d.numel()}, ids.options());
+  const int C = b200_moe_plan_ws_chunks(d.T);
+  auto ws_cnt = at::empty({C, d.E}, ids.options());
+  auto ws_sum = at::empty({C, d.E}, probs.options());
+  auto aux = at::empty({}, probs.options());
+  PlanPtrs q(plan, d);
+  int* p = plan.data_ptr<int>();
+  check(b200_moe_plan(ids.data_ptr<int>(), probs.data_ptr<float>(), d.T, d.E, d.k, d.NT, ws_cnt.data_ptr<int>(),
+                      ws_sum.data_ptr<float>(), p, const_cast<int*>(q.start), const_cast<int*>(q.len),
+                      const_cast<int*>(q.row), const_cast<int*>(q.src), aux.data_ptr<float>(), cur_stream()),
+        "moe_plan", 3);
+  return {plan, aux};
+}
+
+at::Tensor moe_permute(const at::Tensor& x, const at::Tensor& plan, int64_t k, int64_t E) {
+  c10::cuda::CUDAGuard guard(x.device());
+  const MoEDims d(x.size(0), k, E);
+  need_rows(x, "x", d.T, x.size(1));
+  PlanPtrs q(plan, d);
+  auto xp = at::empty({d.Mpad, x.size(1)}, x.options());
+  check(b200_moe_permute(x.data_ptr(), q.tile, q.start, q.len, q.src, d.Mpad, d.k, (int)x.size(1), xp.data_ptr(),
+                         cur_stream()), "moe_permute");
+  return xp;
+}
+
+at::Tensor moe_permute_bwd(const at::Tensor& dxp, const at::Tensor& plan, int64_t T, int64_t k, int64_t E) {
+  c10::cuda::CUDAGuard guard(dxp.device());
+  const MoEDims d(T, k, E);
+  need_rows(dxp, "dx_perm", d.Mpad, dxp.size(1));
+  PlanPtrs q(plan, d);
+  auto dx = at::empty({T, dxp.size(1)}, dxp.options());
+  check(b200_moe_permute_bwd(dxp.data_ptr(), q.row, d.T, d.k, (int)dxp.size(1), dx.data_ptr(), cur_stream()),
+        "moe_permute_bwd");
+  return dx;
+}
+
+at::Tensor moe_combine(const at::Tensor& yp, const at::Tensor& plan, const at::Tensor& wts,
+                       const c10::optional<at::Tensor>& residual, int64_t E) {
+  c10::cuda::CUDAGuard guard(yp.device());
+  need(wts, "weights", at::kFloat);
+  TORCH_CHECK(wts.dim() == 2 && wts.is_contiguous(), "moe_combine: weights [T, k] fp32");
+  const MoEDims d(wts.size(0), wts.size(1), E);
+  need_rows(yp, "y_perm", d.Mpad, yp.size(1));
+  PlanPtrs q(plan, d);
+  const void* r = nullptr;
+  if (residual.has_value()) {
+    need_rows(*residual, "residual", d.T, yp.size(1));
+    r = residual->data_ptr();
+  }
+  auto y = at::empty({d.T, yp.size(1)}, yp.options());
+  check(b200_moe_combine(yp.data_ptr(), q.row, wts.data_ptr<float>(), r, d.T, d.k, (int)yp.size(1), y.data_ptr(),
+                         cur_stream()), "moe_combine");
+  return y;
+}
+
+std::vector<at::Tensor> moe_combine_bwd(const at::Tensor& dy, const at::Tensor& yp, const at::Tensor& plan,
+                                        const at::Tensor& wts, int64_t E) {
+  c10::cuda::CUDAGuard guard(dy.device());
+  need(wts, "weights", at::kFloat);
+  TORCH_CHECK(wts.dim() == 2 && wts.is_contiguous(), "moe_combine_bwd: weights [T, k] fp32");
+  const MoEDims d(wts.size(0), wts.size(1), E);
+  need_rows(dy, "dy", d.T, dy.size(1));
+  need_rows(yp, "y_perm", d.Mpad, dy.size(1));
+  PlanPtrs q(plan, d);
+  auto dyp = at::empty_like(yp);
+  auto dw = at::empty_like(wts);
+  check(b200_moe_combine_bwd(dy.data_ptr(), yp.data_ptr(), wts.data_ptr<float>(), q.tile, q.start, q.len, q.src, d.Mpad,
+                             d.k, (int)dy.size(1), dyp.data_ptr(), dw.data_ptr<float>(), cur_stream()), "moe_combine_bwd");
+  return {dyp, dw};
+}
+
+at::Tensor moe_route_bwd(const at::Tensor& probs, const at::Tensor& ids, const at::Tensor& wts, const at::Tensor& dw,
+                         const at::Tensor& plan, bool norm, double aux_scale) {
+  c10::cuda::CUDAGuard guard(probs.device());
+  need(probs, "probs", at::kFloat);
+  need(ids, "ids", at::kInt);
+  need(wts, "weights", at::kFloat);
+  need(dw, "dw", at::kFloat);
+  TORCH_CHECK(probs.is_contiguous() && ids.is_contiguous() && wts.is_contiguous() && dw.is_contiguous() &&
+              ids.sizes() == wts.sizes() && dw.sizes() == wts.sizes(), "moe_route_bwd: shapes");
+  const MoEDims d(ids.size(0), ids.size(1), probs.size(1));
+  PlanPtrs q(plan, d);
+  auto dl = at::empty({d.T, d.E}, probs.options().dtype(at::kBFloat16));
+  check(b200_moe_route_bwd(probs.data_ptr<float>(), ids.data_ptr<int>(), wts.data_ptr<float>(), dw.data_ptr<float>(),
+                           q.len, d.T, d.E, d.k, norm ? 1 : 0, (float)aux_scale, dl.data_ptr(), cur_stream()),
+        "moe_route_bwd");
+  return dl;
+}
+
+// layout 0 (nt) / 1 (nn): m-grouped, a = the permuted rows [Mpad, K], b = the expert weights [E, rows, cols]; c [Mpad, *].
+// layout 2 (tn): k-grouped wgrad, a [Mpad, M], b [Mpad, N], c [E, M, N].  epi 0 store, 2 accumulate (tn), 5 SwiGLU (nt),
+// 6 SwiGLU backward (nn); the SwiGLU epilogues read set_gemm_swiglu like the dense GEMM.
+void gemm_grouped(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, const at::Tensor& plan, int64_t T, int64_t k,
+                  int64_t layout, int64_t epi) {
+  c10::cuda::CUDAGuard guard(a.device());
+  need(a, "a", at::kBFloat16);
+  need(b, "b", at::kBFloat16);
+  TORCH_CHECK(a.is_contiguous() && b.is_contiguous() && c.is_contiguous(), "gemm_grouped: contiguous operands");
+  TORCH_CHECK(c.scalar_type() == at::kBFloat16 || c.scalar_type() == at::kFloat, "c must be bf16 or fp32");
+  int E, M, N, K;
+  if (layout == 2) {
+    E = c.size(0);
+    M = a.size(1); N = b.size(1); K = a.size(0);
+    TORCH_CHECK(c.dim() == 3 && c.size(1) == M && c.size(2) == N && b.size(0) == K, "gemm_grouped tn: shapes");
+  } else {
+    TORCH_CHECK(b.dim() == 3, "gemm_grouped: expert weights [E, rows, cols]");
+    E = b.size(0);
+    M = a.size(0); K = a.size(1);
+    N = layout == 0 ? b.size(1) : b.size(2);
+    TORCH_CHECK((layout == 0 ? b.size(2) : b.size(1)) == K, "gemm_grouped: K mismatch");
+    TORCH_CHECK(c.dim() == 2 && c.size(0) == M && c.size(1) == (epi == 5 ? N : epi == 6 ? 2 * N : N),
+                "gemm_grouped: c shape");
+  }
+  const MoEDims d(T, k, E);
+  TORCH_CHECK(layout == 2 ? K == d.Mpad : M == d.Mpad, "gemm_grouped: the permuted operand must have ", d.Mpad, " rows");
+  PlanPtrs q(plan, d);
+  const int ldc = layout == 2 ? N : (int)c.stride(0);
+  check(b200_gemm_grouped_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), q.tile, q.start, E, d.Mpad, M, N, K,
+                               (int)a.stride(0), layout == 2 ? (int)b.stride(0) : (int)b.stride(1), ldc, (int)layout,
+                               (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()), "gemm_grouped_bf16");
+}
+
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.doc() = "fms_fsdp_b200 sm_90a kernels";
   m.def("gemm", &gemm);
+  m.def("gemm_grouped", &gemm_grouped);
+  m.def("moe_route", &moe_route);
+  m.def("moe_plan", &moe_plan);
+  m.def("moe_permute", &moe_permute);
+  m.def("moe_permute_bwd", &moe_permute_bwd);
+  m.def("moe_combine", &moe_combine);
+  m.def("moe_combine_bwd", &moe_combine_bwd);
+  m.def("moe_route_bwd", &moe_route_bwd);
   m.def("rmsnorm_fwd", &rmsnorm_fwd);
   m.def("rmsnorm_bwd", &rmsnorm_bwd, py::arg("dy"), py::arg("x"), py::arg("w"), py::arg("rstd"), py::arg("dres") = py::none());
   m.def("add_rmsnorm_fwd", &add_rmsnorm_fwd);

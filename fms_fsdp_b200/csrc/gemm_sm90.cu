@@ -42,6 +42,15 @@ __host__ __device__ constexpr int smem_bytes() {   // ring + 1 KiB alignment sla
 
 enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_ACCUM = 2, EPI_ROPE = 3, EPI_PUSH = 4, EPI_SWIGLU = 5, EPI_SWIGLU_BWD = 6,
        EPI_SCALE = 7 };
+// Grouped (mixture-of-experts) launches of the 128 x 128 kernel carry their mode in the high bits of the EPI template
+// argument, so the instantiations that existed before them keep their names and their code.  Operands live in the
+// expert-sorted row buffer of csrc/moe.cu; the expert weights are one tensor whose rows hold all experts.
+//   GRP_M (forward nt, dgrad nn): m-tile mt belongs to expert p.grp_tile[mt] (-1: past the last segment, the tile is
+//          skipped by producer and consumers alike); B's row (nt) or k (nn) coordinate is offset by e * p.grp_rows.
+//   GRP_K (wgrad tn): problem b0 = expert e of p.nb0; its k-loop covers the rows [start, start + len) of the buffer
+//          (p.grp_seg[e], p.grp_seg[nb0 + e]), rounded out to 64-row blocks that only add padding rows, which are zero;
+//          C of expert e starts at e * p.sc0.
+constexpr int EPI_MASK = 15, GRP_M = 16, GRP_K = 32;
 
 // L2-friendly rasterisation: sweep all n-tiles for a band of GROUP_M m-tiles before moving to the next band, so the
 // band's A rows stay L2-resident while B streams through once per band.
@@ -121,8 +130,11 @@ struct GemmParams {
   long long sc0, sc1;
   // EPI_ROPE (QKV projection): rotate adjacent column pairs of the first rope_cols columns by the angle of
   // (row % rope_S, (col % rope_hd) / 2) before the bf16 store; table is [S][hd/2][cos, sin] fp32 (SURVEY.md K2)
-  const float* rope;
-  int rope_S, rope_hd, rope_cols;
+  // Grouped launches never rotate, so they keep the expert tables in the same slots: grp_tile = the plan's tile table,
+  // grp_rows = weight rows per expert.
+  union { const float* rope; const int* grp_tile; };
+  union { int rope_S; int grp_rows; };
+  int rope_hd, rope_cols;
   // EPI_PUSH (fused wgrad GEMM -> reduce-scatter, SURVEY.md N8): the wgrad tile is not stored to C but pushed over
   // NVLink into the staging buffer of the rank that OWNS that slice of the unit's flat gradient:
   //   e = push_off + row * ldc + col ; owner = e / push_n ; dst = push_bases[owner] + push_rank * push_n + (e - owner * push_n)
@@ -141,8 +153,9 @@ struct GemmParams {
   // aux = the saved projection [M, 2F] and stores d(gate) | d(up) to C [M, 2F] -- dS itself never reaches memory.
   void* aux;
   int ld_aux, swi_F, swi_gate_first;
-  // EPI_SCALE (fp8 e4m3 operands, FP8 = true): C = acc * scale_a[row] * scale_b[col]
-  const float* scale_a;
+  // EPI_SCALE (fp8 e4m3 operands, FP8 = true): C = acc * scale_a[row] * scale_b[col].  GRP_K: grp_seg = the plan's
+  // [start | len] of every expert.
+  union { const float* scale_a; const int* grp_seg; };
   const float* scale_b;
 };
 
@@ -259,7 +272,11 @@ __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p,
                 AgParams ag) {
   static_assert(!FP8 || (!A_MN && !B_MN && !AG && !BATCH), "fp8 operands: K-major (nt) only");
-  constexpr int NST = ring_stages<EPI>();
+  constexpr int EP = EPI & EPI_MASK;                            // the epilogue
+  constexpr bool GM = (EPI & GRP_M) != 0, GK = (EPI & GRP_K) != 0;
+  static_assert(!(GM || GK) || (!AG && !FP8 && !BATCH && EP != EPI_PUSH), "grouped: no comm, fp8, batch or push");
+  static_assert(!GK || (A_MN && B_MN), "k-grouped: wgrad (tn) only");
+  constexpr int NST = ring_stages<EP>();
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B atoms must sit on 1024 B boundaries
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -272,7 +289,7 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   constexpr int BKE = FP8 ? 2 * BK : BK;
   const int num_kb = (p.K + BKE - 1) / BKE;
   const int tiles_per_problem = p.m_tiles * p.n_tiles;
-  const int num_tiles = BATCH ? tiles_per_problem * p.nb0 * p.nb1 : tiles_per_problem;
+  const int num_tiles = (BATCH || GK) ? tiles_per_problem * p.nb0 * p.nb1 : tiles_per_problem;
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
@@ -287,12 +304,22 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
   auto coords = [&](int t, int& mt, int& nt, int& b0, int& b1) {
     b0 = b1 = 0;
-    if constexpr (BATCH) {
+    if constexpr (BATCH || GK) {
       const int prob = t / tiles_per_problem;
       b0 = prob % p.nb0; b1 = prob / p.nb0;
       tile_coords(t - prob * tiles_per_problem, p.m_tiles, p.n_tiles, mt, nt);
     } else {
       tile_coords((t + p.tile_rot) % num_tiles, p.m_tiles, p.n_tiles, mt, nt);
+    }
+  };
+  // grouped modes: the expert of an m-tile (GRP_M, -1 = skip the tile) and the k-blocks of a problem (GRP_K)
+  auto group = [&](int mt, int b0, int& e, int& kb0, int& kb1) {
+    e = 0; kb0 = 0; kb1 = num_kb;
+    if constexpr (GM) e = p.grp_tile[mt];
+    if constexpr (GK) {
+      const int s = p.grp_seg[b0];
+      kb0 = s / BKE;
+      kb1 = (s + p.grp_seg[p.nb0 + b0] + BKE - 1) / BKE;
     }
   };
 
@@ -302,17 +329,21 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       int stage = 0;
       uint32_t phase = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int mt, nt, b0, b1;
+        int mt, nt, b0, b1, e, kb0, kb1;
         coords(t, mt, nt, b0, b1);
+        group(mt, b0, e, kb0, kb1);
+        if (e < 0) continue;
         const int m0 = mt * BM;
+        // GRP_M: the expert's slab of the weight rows -- B's rows (K-major) or k-rows (MN-major)
+        const int bn = (GM && !B_MN) ? e * p.grp_rows : 0, bk = (GM && B_MN) ? e * p.grp_rows : 0;
         // B rows of the two 64-row halves of the tile (SwiGLU: the same features of both halves of the fused weight)
-        const int n0 = (EPI == EPI_SWIGLU) ? nt * 64 : nt * BN;
-        const int n1 = (EPI == EPI_SWIGLU) ? nt * 64 + p.swi_F : n0 + 64;
+        const int n0 = ((EP == EPI_SWIGLU) ? nt * 64 : nt * BN) + bn;
+        const int n1 = (EP == EPI_SWIGLU) ? n0 + p.swi_F : n0 + 64;
         auto load = [&](void* dst, const CUtensorMap* tm, int c0, int c1) {
           if constexpr (BATCH) tma_load_4d(dst, tm, &full_bar[stage], c0, c1, b0, b1);
           else tma_load_2d(dst, tm, &full_bar[stage], c0, c1);
         };
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1);
           uint8_t* sa = smem + stage * STAGE_BYTES;
           uint8_t* sb = sa + A_BYTES;
@@ -341,8 +372,8 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             load(sb, &tmB, k0, n0);                                    // boxes {64 k, 64 rows}
             load(sb + 64 * BK * 2, &tmB, k0, n1);
           } else {
-            load(sb, &tmB, n0, k0);                                    // boxes {64 n, 64 k-rows}
-            load(sb + 64 * BK * 2, &tmB, n0 + 64, k0);
+            load(sb, &tmB, n0, k0 + bk);                               // boxes {64 n, 64 k-rows}
+            load(sb + 64 * BK * 2, &tmB, n0 + 64, k0 + bk);
           }
           if (++stage == NST) { stage = 0; phase ^= 1; }
         }
@@ -397,13 +428,15 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     int stage = 0;
     uint32_t phase = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int mt, nt, b0, b1;
+      int mt, nt, b0, b1, e, kb0, kb1;
       coords(t, mt, nt, b0, b1);
+      group(mt, b0, e, kb0, kb1);
+      if (e < 0) continue;
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.f;
       int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      for (int kb = kb0; kb < kb1; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_u32(smem + stage * STAGE_BYTES) + cw * (64 * 128);   // this warpgroup's 64 rows / box
         const uint32_t sb = smem_u32(smem + stage * STAGE_BYTES) + A_BYTES;
@@ -432,10 +465,10 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
       // ---- epilogue: thread holds rows r and r + 8, column pairs 8 j + 2 (lane & 3) for j = 0..15
       size_t boff = 0;
-      if constexpr (BATCH) boff = (size_t)b0 * p.sc0 + (size_t)b1 * p.sc1;
+      if constexpr (BATCH || GK) boff = (size_t)b0 * p.sc0 + (size_t)b1 * p.sc1;
       const int rbase = mt * BM + cw * 64 + w4 * 16 + (lane >> 2);
       const int cq = 2 * (lane & 3);
-      if constexpr (EPI == EPI_PUSH) {
+      if constexpr (EP == EPI_PUSH) {
         if (p.push_bulk) {
           uint8_t* stg = push_stage + cw * 64 * PUSH_PITCH;
           asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // own bulk stores of the last tile have read
@@ -467,9 +500,9 @@ gemm_bf16_wgmma(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           continue;
         }
       }
-      epilogue_tile<EPI, OutT, BN / 8>(p, acc, boff, rbase, nt, cq);
+      epilogue_tile<EP, OutT, BN / 8>(p, acc, boff, rbase, nt, cq);
     }
-    if constexpr (EPI == EPI_PUSH) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // every pushed row is out
+    if constexpr (EP == EPI_PUSH) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // every pushed row is out
   }
 }
 
@@ -483,7 +516,7 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
     if (e != cudaSuccess) return (int)e;
     configured = true;
   }
-  long long tiles = (long long)p.m_tiles * p.n_tiles * (BATCH ? (long long)p.nb0 * p.nb1 : 1);
+  long long tiles = (long long)p.m_tiles * p.n_tiles * ((BATCH || (EPI & GRP_K)) ? (long long)p.nb0 * p.nb1 : 1);
   // the comm warps of ALL SMs carry the fused gather, so that launch always covers the full machine
   int grid = (!AG && tiles < sm_count()) ? (int)tiles : sm_count();
   if (grid < 1) grid = 1;
@@ -818,6 +851,64 @@ extern "C" int b200_bgemm_bf16(const void* A, const void* B, void* C, int M, int
   }
   if (b_mn) return dispatch_batched<false, true>(tmA, tmB, p, epi, out_fp32, stream);
   return dispatch_batched<false, false>(tmA, tmB, p, epi, out_fp32, stream);
+}
+
+// Grouped GEMM over the expert-sorted rows of csrc/moe.cu, 128 x 128 tiles.  tile / seg: the plan's tile table and
+// [start | len] of the E experts; Mpad: rows of the permuted buffer (a multiple of 128).  lda / ldb / ldc: row strides.
+//   layout 0 (nt, GRP_M): C[Mpad, N] = A[Mpad, K] W_e[N, K]^T, B = W [E N, K].  epi store, or SwiGLU (N = 2F rows of
+//                  the expert's fused [gate | up]; C = the projection [Mpad, 2F], aux = silu(gate) up [Mpad, F])
+//   layout 1 (nn, GRP_M): C[Mpad, N] = A[Mpad, K] W_e[K, N], B = W [E K, N].  epi store, or SwiGLU backward (C = the
+//                  projection's gradient [Mpad, 2N], aux = the projection)
+//   layout 2 (tn, GRP_K): C[e] = A_e^T B_e [M, N] over the rows of expert e, A [Mpad, M], B [Mpad, N], C [E, M, N]
+//                  contiguous.  epi store or accumulate, bf16 or fp32 output.
+extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, const int* tile, const int* seg, int E,
+                                      int Mpad, int M, int N, int K, int lda, int ldb, int ldc, int layout, int epi,
+                                      int out_fp32, cudaStream_t stream) {
+  using namespace b200;
+  if (E < 1 || Mpad % BM || (N % 8) || (K % 8) || (M % 8)) return -14;
+  CUtensorMap tmA, tmB;
+  const AgParams ag{};
+  if (layout == 2) {
+    if (epi != EPI_STORE && epi != EPI_ACCUM) return -14;
+    if (make_tmap_2d_bf16(&tmA, A, (uint64_t)M, (uint64_t)Mpad, (uint64_t)lda, 64, BK)) return 1001;
+    if (make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)Mpad, (uint64_t)ldb, 64, BK)) return 2001;
+    GemmParams p = make_params(C, nullptr, M, N, Mpad, ldc, 0, epi);
+    p.nb0 = E; p.nb1 = 1; p.sc0 = (long long)M * N; p.sc1 = 0;
+    p.grp_seg = seg;
+    constexpr int G = GRP_K;
+    if (out_fp32) {
+      if (epi == EPI_ACCUM) return launch<true, true, G | EPI_ACCUM, float, false>(tmA, tmB, p, ag, stream);
+      return launch<true, true, G | EPI_STORE, float, false>(tmA, tmB, p, ag, stream);
+    }
+    if (epi == EPI_ACCUM) return launch<true, true, G | EPI_ACCUM, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    return launch<true, true, G | EPI_STORE, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+  }
+  if (out_fp32 || M != Mpad) return -14;
+  if (make_tmap_2d_bf16(&tmA, A, (uint64_t)K, (uint64_t)Mpad, (uint64_t)lda, BK, BM)) return 1001;
+  GemmParams p = make_params(C, nullptr, Mpad, N, K, ldc, 0, epi);
+  p.grp_tile = tile;
+  constexpr int G = GRP_M;
+  if (layout == 0) {
+    if (make_tmap_2d_bf16(&tmB, B, (uint64_t)K, (uint64_t)E * N, (uint64_t)ldb, BK, 64)) return 2001;
+    p.grp_rows = N;
+    if (epi == EPI_SWIGLU) {
+      if (!p.aux || p.swi_F <= 0 || N != 2 * p.swi_F || (p.swi_F % 64) || (p.ld_aux % 8)) return -11;
+      p.N = p.swi_F;
+      p.n_tiles = p.swi_F / 64;
+      return launch<false, false, G | EPI_SWIGLU, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+    }
+    if (epi != EPI_STORE) return -14;
+    return launch<false, false, G | EPI_STORE, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+  }
+  if (layout != 1) return -14;
+  if (make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)E * K, (uint64_t)ldb, 64, BK)) return 2001;
+  p.grp_rows = K;
+  if (epi == EPI_SWIGLU_BWD) {
+    if (!p.aux || p.swi_F != N || (p.ld_aux % 8)) return -12;
+    return launch<false, true, G | EPI_SWIGLU_BWD, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
+  }
+  if (epi != EPI_STORE) return -14;
+  return launch<false, true, G | EPI_STORE, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
 }
 
 // GEMM + fused all-gather.  Supported: bf16 output, EPI store|residual|rope|swiglu (nt), store|residual|swiglu_bwd (nn),

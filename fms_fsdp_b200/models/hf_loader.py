@@ -36,7 +36,10 @@ _REFUSED_MODEL_TYPES = {
     "olmo2": "q / k RMSNorm over the whole projection instead of per head",
     "olmo3": "q / k RMSNorm over the whole projection instead of per head",
     "qwen2": "q / k / v projection biases",
+    # the engine trains these feed-forwards (LLaMAConfig.moe_num_experts) but does not import their checkpoints yet;
+    # Mixtral is refused by convert_hf_state_dict instead (its attention config also serves the frozen speculator base)
     "qwen3_moe": "sparse mixture-of-experts feed-forward",
+    "qwen2_moe": "shared experts and q / k / v projection biases",
 }
 
 
@@ -104,6 +107,9 @@ def _read_hf_tensors(model_path: str) -> Dict[str, torch.Tensor]:
 
 
 def convert_hf_state_dict(hf: Dict[str, torch.Tensor], cfg: LLaMAConfig) -> Dict[str, torch.Tensor]:
+    if any(".block_sparse_moe." in n or ".mlp.experts." in n or n.endswith(".mlp.gate.weight") for n in hf):
+        raise NotImplementedError("mixture-of-experts checkpoints (Mixtral, Qwen3-MoE) are not imported for training yet; "
+                                  "Llama and Qwen3 dense checkpoints are")
     sd = {"shared.emb.weight": hf["model.embed_tokens.weight"],
           "shared.head.weight": hf.get("lm_head.weight", hf["model.embed_tokens.weight"]),
           "dec_norm.weight": hf["model.norm.weight"]}

@@ -57,11 +57,29 @@ class LLaMAConfig:
     # extension (not an fms field): head dimension when it is not emb_dim // nheads (Qwen3-0.6B / 4B: 128 with
     # emb_dim / nheads = 64 / 80).  None = emb_dim // nheads.
     attn_head_dim: Optional[int] = None
+    # extension (not an fms field): sparse mixture-of-experts feed-forward (Qwen3-MoE, Mixtral).  moe_num_experts > 0
+    # replaces every block's ``ff_sub_layer`` with ``moe``: router ``moe.gate.weight`` [E, D] and SwiGLU experts
+    # ``moe.w1`` [E, 2F, D] ([gate | up] per expert) and ``moe.w2`` [E, D, F], F = moe_hidden_dim.  Each token goes to
+    # its moe_top_k experts (dropless), weighted by their router probabilities, renormalised when moe_norm_topk.
+    # moe_aux_loss_coef scales the Switch load-balancing loss coef * mean_layers(E * sum_e f_e * P_e), computed per layer
+    # (HF instead concatenates all layers' router logits before taking the means).
+    moe_num_experts: int = 0
+    moe_top_k: int = 2
+    moe_hidden_dim: int = 0
+    moe_norm_topk: bool = True
+    moe_aux_loss_coef: float = 0.0
 
     @property
     def hidden_dim(self) -> int:
         return self.multiple_of * ((int(self.hidden_grow_factor * self.emb_dim) + self.multiple_of - 1)
                                    // self.multiple_of)
+
+    def inactive_params(self) -> int:
+        """Expert parameters a token does not use: (E - k) experts per block (0 for a dense model).  Model FLOPs per
+        token count the active parameters only."""
+        if self.moe_num_experts <= 0:
+            return 0
+        return self.nlayers * (self.moe_num_experts - self.moe_top_k) * 3 * self.emb_dim * self.moe_hidden_dim
 
     @property
     def kv_heads(self) -> int:
@@ -178,6 +196,31 @@ class GatedLinearUnit(nn.Module):
             nn.init.trunc_normal_(w, mean=0.0, std=0.02)
 
 
+class MoEFeedForward(nn.Module):
+    """Router + SwiGLU experts; the weights of all experts are single tensors (``ops.moe_mlp``)."""
+
+    def __init__(self, cfg: LLaMAConfig, device=None, dtype=None):
+        super().__init__()
+        E, F, D = cfg.moe_num_experts, cfg.moe_hidden_dim, cfg.emb_dim
+        self.config = cfg
+        self.gate = _Weight(E, D, device, dtype)
+        self.w1 = nn.Parameter(torch.empty(E, 2 * F, D, device=device, dtype=dtype))
+        self.w2 = nn.Parameter(torch.empty(E, D, F, device=device, dtype=dtype))
+        self.last_aux = None          # the load-balancing statistic of the last forward (device scalar)
+
+    def reset_parameters(self):
+        for w in (self.gate.weight, self.w1, self.w2):
+            nn.init.trunc_normal_(w, mean=0.0, std=0.02)
+
+    def forward(self, h, residual):
+        cfg = self.config
+        # the loss is the mean over layers: each block's share of the coefficient (read here, so that the gradient and
+        # LLaMA.moe_aux_loss() always use the same value)
+        y, self.last_aux = ops.moe_mlp(h, self.gate.weight, self.w1, self.w2, cfg.moe_top_k, cfg.moe_norm_topk,
+                                       cfg.moe_aux_loss_coef / cfg.nlayers, residual=residual)
+        return y
+
+
 class WordEmbedding(nn.Module):
     """Embedding + reversible (untied unless tie_heads) output head: ``shared.emb`` / ``shared.head``."""
 
@@ -214,7 +257,10 @@ class LLaMABlock(nn.Module):
         self.ln = RMSNorm(cfg.emb_dim, cfg.norm_eps, device, dtype)
         self.ff_ln = RMSNorm(cfg.emb_dim, cfg.norm_eps, device, dtype)
         self.attn = MultiHeadAttention(cfg, device, dtype)
-        self.ff_sub_layer = GatedLinearUnit(cfg, device, dtype)
+        if cfg.moe_num_experts > 0:
+            self.moe = MoEFeedForward(cfg, device, dtype)
+        else:
+            self.ff_sub_layer = GatedLinearUnit(cfg, device, dtype)
         object.__setattr__(self, "_rot", rot_emb)  # shared, not a submodule (no params, not in state dict)
 
     def forward(self, x, doc=None):
@@ -228,6 +274,9 @@ class LLaMABlock(nn.Module):
                                 a.head_dim, doc=doc, qk_norm=a.qk_norm_args())
         x = a.dense(ctx, residual=x)
         h, x = self.ff_ln.fork(x)
+        if cfg.moe_num_experts > 0:
+            x = self.moe(h, x)
+            return x if doc is None else (x, doc)
         ff = self.ff_sub_layer
         # gate/up GEMM with the SwiGLU epilogue, down projection with the residual epilogue: one autograd node
         x = ops.gated_mlp(h, ff.wg1_fused.weight, ff.w2.weight, residual=x)
@@ -253,6 +302,13 @@ class LLaMA(nn.Module):
     def get_config(self) -> LLaMAConfig:
         return self.config
 
+    def moe_aux_loss(self):
+        """coef * mean over layers of the load-balancing statistic of the last forward, as a device scalar (its
+        gradient is already part of the backward); None for a dense model or before the first forward."""
+        if self.config.moe_num_experts <= 0 or self.layers[0].moe.last_aux is None:
+            return None
+        return torch.stack([blk.moe.last_aux for blk in self.layers]).mean() * self.config.moe_aux_loss_coef
+
     def reset_parameters(self):
         self.shared.reset_parameters()
         self.dec_norm.reset_parameters()
@@ -260,7 +316,7 @@ class LLaMA(nn.Module):
             blk.ln.reset_parameters()
             blk.ff_ln.reset_parameters()
             blk.attn.reset_parameters()
-            blk.ff_sub_layer.reset_parameters()
+            (blk.moe if self.config.moe_num_experts > 0 else blk.ff_sub_layer).reset_parameters()
 
     # ---- plain (unsharded) forward: logits, as the reference model returns
     def forward(self, x, labels=None, return_hidden: bool = False):

@@ -275,6 +275,77 @@ def gated_down_bwd(dy, w2, gu, gate_first=True):
     return dgu
 
 
+# ----------------------------------------------------------------------- mixture of experts (csrc/moe.cu)
+# Semantics and the plan layout: torch_kernels (the oracle).  No fallback: an unsupported shape or dtype raises.
+moe_rows = torch_kernels.moe_rows
+moe_plan_views = torch_kernels.moe_plan_views
+
+
+def moe_route(logits, top_k, norm_topk):
+    ids, wts, probs = _C.moe_route(logits.float().contiguous(), int(top_k), bool(norm_topk))
+    return ids, wts, probs
+
+
+def moe_plan(ids, probs):
+    plan, aux = _C.moe_plan(ids, probs)
+    return plan, aux
+
+
+def moe_permute(x, plan, k, E):
+    return _C.moe_permute(x.contiguous(), plan, int(k), int(E))
+
+
+def moe_permute_bwd(dxp, plan, T, k, E):
+    return _C.moe_permute_bwd(dxp, plan, int(T), int(k), int(E))
+
+
+def moe_combine(yp, plan, wts, residual, E):
+    return _C.moe_combine(yp, plan, wts, None if residual is None else residual.contiguous(), int(E))
+
+
+def moe_combine_bwd(dy, yp, plan, wts, E):
+    dyp, dw = _C.moe_combine_bwd(dy.contiguous(), yp, plan, wts, int(E))
+    return dyp, dw
+
+
+def moe_route_bwd(probs, ids, wts, dw, plan, norm_topk, aux_scale):
+    """dlogits in bf16: the operand of the router's dgrad and wgrad GEMMs."""
+    return _C.moe_route_bwd(probs, ids, wts, dw, plan, bool(norm_topk), float(aux_scale))
+
+
+def moe_up_fwd(xp, w1, plan, T, k):
+    F = w1.shape[1] // 2
+    h = torch.empty(xp.shape[0], 2 * F, dtype=torch.bfloat16, device=xp.device)
+    s = torch.empty(xp.shape[0], F, dtype=torch.bfloat16, device=xp.device)
+    _C.set_gemm_swiglu(s, F, True)
+    _C.gemm_grouped(xp, w1.contiguous(), h, plan, int(T), int(k), 0, 5)
+    return h, s
+
+
+def moe_down_fwd(sp, w2, plan, T, k):
+    y = torch.empty(sp.shape[0], w2.shape[1], dtype=torch.bfloat16, device=sp.device)
+    _C.gemm_grouped(sp, w2.contiguous(), y, plan, int(T), int(k), 0, 0)
+    return y
+
+
+def moe_down_bwd(dyp, w2, hp, plan, T, k):
+    dh = torch.empty_like(hp)
+    _C.set_gemm_swiglu(hp, w2.shape[2], True)
+    _C.gemm_grouped(dyp, w2.contiguous(), dh, plan, int(T), int(k), 1, 6)
+    return dh
+
+
+def moe_up_dgrad(dhp, w1, plan, T, k):
+    dx = torch.empty(dhp.shape[0], w1.shape[2], dtype=torch.bfloat16, device=dhp.device)
+    _C.gemm_grouped(dhp, w1.contiguous(), dx, plan, int(T), int(k), 1, 0)
+    return dx
+
+
+def moe_wgrad(a, b, plan, T, k, out, accumulate=False):
+    _C.gemm_grouped(a, b, out, plan, int(T), int(k), 2, 2 if accumulate else 0)
+    return out
+
+
 # ------------------------------------------------------------------------ optional fp8 (e4m3) forward GEMMs
 def quant_rowwise_e4m3(x):
     if x.dtype != torch.bfloat16 or x.dim() != 2 or x.shape[1] % 16 or x.stride(-1) != 1:

@@ -497,6 +497,67 @@ def gated_mlp(x, wg1, w2, residual: Optional[torch.Tensor] = None, gate_first: b
     return _GatedMLP.apply(x, wg1, w2, residual, gate_first)
 
 
+class _MoEMLP(torch.autograd.Function):
+    """Dropless top-k mixture of SwiGLU experts as ONE node.  Forward: router GEMM (fp32 logits), route, plan, permute,
+    the m-grouped gate/up GEMM with the SwiGLU epilogue, the m-grouped down GEMM, combine (+ residual).  Backward: the
+    mirror image, with the load-balancing loss's gradient added inside the routing backward.  Every step is
+    deterministic, so a recomputed forward routes exactly as the first one did."""
+
+    @staticmethod
+    def forward(ctx, h, router_w, w1, w2, residual, top_k, norm_topk, aux_coef):
+        K = kernels_for(h)
+        D = h.shape[-1]
+        h2 = h.reshape(-1, D)
+        T = h2.shape[0]
+        wr = _wdata(router_w)
+        E = wr.shape[0]
+        logits = K.gemm(h2, wr, "nt", out_dtype=torch.float32)
+        ids, wts, probs = K.moe_route(logits, top_k, norm_topk)
+        plan, aux = K.moe_plan(ids, probs)
+        xp = K.moe_permute(h2, plan, top_k, E)
+        hp, sp = K.moe_up_fwd(xp, _wdata(w1), plan, T, top_k)
+        yp = K.moe_down_fwd(sp, _wdata(w2), plan, T, top_k)
+        y = K.moe_combine(yp, plan, wts, None if residual is None else residual.reshape(-1, D), E)
+        ctx.K, ctx.ws, ctx.has_res = K, (router_w, w1, w2), residual is not None
+        ctx.args = (T, E, top_k, norm_topk, aux_coef * E / (T * T))
+        ctx.save_for_backward(h, ids, wts, probs, plan, xp, hp, sp, yp)
+        ctx.mark_non_differentiable(aux)
+        return y.view(h.shape), aux
+
+    @staticmethod
+    def backward(ctx, dy, _daux):
+        h, ids, wts, probs, plan, xp, hp, sp, yp = ctx.saved_tensors
+        K, (router_w, w1, w2) = ctx.K, ctx.ws
+        T, E, k, norm_topk, aux_scale = ctx.args
+        h2 = h.reshape(T, -1)
+        dyp, dw = K.moe_combine_bwd(dy.reshape(T, -1), yp, plan, wts, E)
+        dhp = K.moe_down_bwd(dyp, _wdata(w2), hp, plan, T, k)
+        dw2 = _deliver_wgrad(w2, lambda out, acc: K.moe_wgrad(dyp, sp, plan, T, k, out, acc)) \
+            if ctx.needs_input_grad[3] else None
+        dxp = K.moe_up_dgrad(dhp, _wdata(w1), plan, T, k)
+        dw1 = _deliver_wgrad(w1, lambda out, acc: K.moe_wgrad(dhp, xp, plan, T, k, out, acc)) \
+            if ctx.needs_input_grad[2] else None
+        dh = K.moe_permute_bwd(dxp, plan, T, k, E)
+        dl = K.moe_route_bwd(probs, ids, wts, dw, plan, norm_topk, aux_scale).to(h.dtype)
+        dh = K.gemm(dl, _wdata(router_w), "nn", residual=dh).view_as(h)
+        dwr = _deliver_wgrad(router_w, lambda out, acc: K.gemm(dl, h2, "tn", out=out, accumulate=acc)) \
+            if ctx.needs_input_grad[1] else None
+        return dh, dwr, dw1, dw2, (dy if ctx.has_res else None), None, None, None
+
+
+def moe_mlp(h, router_w, w1, w2, top_k, norm_topk=False, aux_coef=0.0, residual: Optional[torch.Tensor] = None):
+    """Dropless top-k mixture of SwiGLU experts: ``residual + sum_s w_s * expert_{e_s}(h)`` per token.
+
+    router_w [E, D]; w1 [E, 2F, D] (each expert's [gate | up], like ``wg1_fused``); w2 [E, D, F].  Routing: fp32 softmax
+    of ``h @ router_w^T``, the ``top_k`` experts by logit (ties to the lower index), weights = their probabilities,
+    renormalised to sum to 1 when ``norm_topk``.  Returns ``(y, aux)`` with aux = E * sum_e (count_e / T) * mean_t p_te,
+    the Switch load-balancing statistic of this call (a detached fp32 scalar on the device).  Its gradient, scaled by
+    ``aux_coef``, is added to the router's in backward: callers do not add ``aux`` to their loss."""
+    if _GEMM_PRECISION == "fp8":
+        raise NotImplementedError("moe_mlp: the grouped expert GEMMs are bf16 only")
+    return _MoEMLP.apply(h, router_w, w1, w2, residual, int(top_k), bool(norm_topk), float(aux_coef))
+
+
 class _AddRMSNorm(torch.autograd.Function):
     """residual_out = residual + x (kept in the residual stream dtype, fp32 for Mamba);
     y = rmsnorm(residual_out) in x.dtype.  (mamba_ssm fused_add_norm, SURVEY.md M6.)"""

@@ -327,6 +327,170 @@ def swiglu_bwd(ds, gu, gate_first=True):
 
 
 # ----------------------------------------------------------------------------------------------
+# Mixture of experts, dropless (csrc/moe.cu).  T tokens, E experts, top-k.  Each (token t, slot s) -- entry i = t k + s --
+# gets a row of the expert-sorted ("permuted") buffer: expert e owns the segment [start_e, start_e + len_e), padded to a
+# multiple of 128 rows, in (token, slot) order.  The buffer has the worst-case Mpad = round_up(T k + 127 E, 128) rows so
+# that no size ever has to reach the host; 128-row tiles past the last segment belong to no expert (-1).  The plan is one
+# int32 tensor [tile NT | start E | len E | row T k | src Mpad].  Padding rows of every permuted operand are zero.
+# ----------------------------------------------------------------------------------------------
+def moe_rows(T, k, E):
+    """(Mpad, NT): rows of the permuted buffer and its number of 128-row tiles."""
+    Mpad = (T * k + 127 * E + 127) // 128 * 128
+    return Mpad, Mpad // 128
+
+
+def moe_plan_views(plan, T, k, E):
+    """(tile [NT], start [E], len [E], row [T, k], src [Mpad]) views of a plan."""
+    Mpad, NT = moe_rows(T, k, E)
+    tile, start, length, row, src = torch.split(plan, [NT, E, E, T * k, Mpad])
+    return tile, start, length, row.view(T, k), src
+
+
+def moe_route(logits, top_k, norm_topk):
+    """fp32 softmax of the router logits [T, E]; the top-k experts by logit (NaN ranks as -inf), ties to the lower
+    index; their probabilities as weights, renormalised to sum to 1 (in slot order) when ``norm_topk``.
+    Returns (ids [T, k] int32, weights [T, k] fp32, probs [T, E] fp32)."""
+    lf = logits.float()
+    probs = torch.softmax(lf, dim=-1)
+    # selection sees NaN as -inf (k distinct experts in [0, E) whatever the logits); the NaN still reaches the weights
+    key = torch.where(torch.isnan(lf), torch.full_like(lf, -float("inf")), lf)
+    ids = torch.sort(key, dim=-1, descending=True, stable=True).indices[:, :top_k]
+    w = probs.gather(1, ids)
+    if norm_topk:
+        tot = w[:, 0].clone()
+        for s in range(1, top_k):
+            tot = tot + w[:, s]
+        w = w / tot[:, None]
+    return ids.to(torch.int32), w, probs
+
+
+def moe_plan(ids, probs):
+    """(plan, aux): the plan of the routing ``ids`` and the load-balancing statistic
+    aux = E * sum_e (count_e / T) * mean_t probs[t, e] (fp32 scalar)."""
+    T, k = ids.shape
+    E = probs.shape[1]
+    Mpad, NT = moe_rows(T, k, E)
+    flat = ids.reshape(-1).long()
+    count = torch.bincount(flat, minlength=E)
+    padded = (count + 127) // 128 * 128
+    start = torch.cumsum(padded, 0) - padded
+    order = torch.sort(flat, stable=True).indices            # by expert, (token, slot) order inside
+    se = flat[order]
+    first = torch.cumsum(count, 0) - count
+    row = torch.empty(T * k, dtype=torch.long, device=ids.device)
+    row[order] = start[se] + torch.arange(T * k, device=ids.device) - first[se]
+    src = torch.full((Mpad,), -1, dtype=torch.long, device=ids.device)
+    src[row] = torch.arange(T * k, device=ids.device)
+    r = torch.arange(NT, device=ids.device) * 128
+    tile = torch.where(r < padded.sum(), torch.searchsorted(start, r, right=True) - 1, torch.full_like(r, -1))
+    plan = torch.cat([tile, start, count, row, src]).to(torch.int32)
+    aux = (count.float() * probs.float().sum(0)).sum() * E / (T * T)
+    return plan, aux
+
+
+def moe_permute(x, plan, k, E):
+    """X_perm [Mpad, D]: x[t] in the rows of its k entries, zero elsewhere."""
+    T, D = x.shape
+    row = moe_plan_views(plan, T, k, E)[3].long()
+    xp = torch.zeros(moe_rows(T, k, E)[0], D, dtype=x.dtype, device=x.device)
+    xp[row.reshape(-1)] = x.repeat_interleave(k, 0)
+    return xp
+
+
+def moe_permute_bwd(dxp, plan, T, k, E):
+    """dx[t] = sum_s dX_perm[row(t, s)], fp32 in slot order."""
+    row = moe_plan_views(plan, T, k, E)[3].long()
+    acc = dxp[row[:, 0]].float()
+    for s in range(1, k):
+        acc = acc + dxp[row[:, s]].float()
+    return acc.to(dxp.dtype)
+
+
+def moe_combine(yp, plan, wts, residual, E):
+    """y[t] = residual[t] + sum_s w[t, s] Y_perm[row(t, s)], fp32 in slot order."""
+    T, k = wts.shape
+    row = moe_plan_views(plan, T, k, E)[3].long()
+    acc = residual.float() if residual is not None else torch.zeros(T, yp.shape[1], device=yp.device)
+    for s in range(k):
+        acc = acc + wts[:, s:s + 1].float() * yp[row[:, s]].float()
+    return acc.to(yp.dtype)
+
+
+def moe_combine_bwd(dy, yp, plan, wts, E):
+    """(dY_perm [Mpad, D] = w dy[t] in the routed rows, zero elsewhere;  dw [T, k] = <dy[t], Y_perm[row]>)."""
+    T, k = wts.shape
+    row = moe_plan_views(plan, T, k, E)[3].long().reshape(-1)
+    dyk = dy.float().repeat_interleave(k, 0)
+    dyp = torch.zeros_like(yp)
+    dyp[row] = (wts.reshape(-1, 1).float() * dyk).to(yp.dtype)
+    dw = (dyk * yp[row].float()).sum(-1).view(T, k)
+    return dyp, dw
+
+
+def moe_route_bwd(probs, ids, wts, dw, plan, norm_topk, aux_scale):
+    """dlogits [T, E] (fp32) of the routing weights' gradient ``dw``, through the renormalisation and the softmax, plus
+    the load-balancing gradient: aux_scale * count_e on every probability of expert e."""
+    T, k = ids.shape
+    E = probs.shape[1]
+    count = moe_plan_views(plan, T, k, E)[2]
+    il = ids.long()
+    p = probs.float()
+    g = dw.float()
+    if norm_topk:
+        z = p.gather(1, il).sum(1, keepdim=True)
+        g = (g - (g * wts.float()).sum(1, keepdim=True)) / z
+    dp = torch.zeros_like(p).scatter_add_(1, il, g) + aux_scale * count.float()[None]
+    return p * (dp - (p * dp).sum(1, keepdim=True))
+
+
+def _segments(plan, T, k, E):
+    _, start, length, _, _ = moe_plan_views(plan, T, k, E)
+    return [(s, n, (n + 127) // 128 * 128) for s, n in zip(start.tolist(), length.tolist())]
+
+
+def _grouped_m(a, w, plan, T, k, layout, ncols):
+    """m-grouped product over each expert's whole (padded) segment; rows of no expert stay zero."""
+    E = w.shape[0]
+    c = torch.zeros(a.shape[0], ncols, dtype=a.dtype, device=a.device)
+    for e, (s, _, n) in enumerate(_segments(plan, T, k, E)):
+        if n:
+            c[s:s + n] = gemm(a[s:s + n], w[e], layout)
+    return c
+
+
+def moe_up_fwd(xp, w1, plan, T, k):
+    """Expert gate/up projections with SwiGLU: (H [Mpad, 2F] = X_perm W1_e^T, silu(gate) * up [Mpad, F]).
+    w1: [E, 2F, D], each expert's [gate | up]."""
+    h = _grouped_m(xp, w1, plan, T, k, "nt", w1.shape[1])
+    return h, swiglu_fwd(h, True)
+
+
+def moe_down_fwd(sp, w2, plan, T, k):
+    """Y_perm [Mpad, D] = S_perm W2_e^T, w2: [E, D, F]."""
+    return _grouped_m(sp, w2, plan, T, k, "nt", w2.shape[1])
+
+
+def moe_down_bwd(dyp, w2, hp, plan, T, k):
+    """d(H) [Mpad, 2F] = swiglu_bwd(dY_perm W2_e, H)."""
+    return swiglu_bwd(_grouped_m(dyp, w2, plan, T, k, "nn", w2.shape[2]), hp, True)
+
+
+def moe_up_dgrad(dhp, w1, plan, T, k):
+    """dX_perm [Mpad, D] = dH W1_e."""
+    return _grouped_m(dhp, w1, plan, T, k, "nn", w1.shape[2])
+
+
+def moe_wgrad(a, b, plan, T, k, out, accumulate=False):
+    """out[e] (+)= A_e^T B_e over the routed rows of expert e (out [E, M, N]); an expert with no rows gets zeros."""
+    for e, (s, n, _) in enumerate(_segments(plan, T, k, out.shape[0])):
+        if n:
+            gemm(a[s:s + n], b[s:s + n], "tn", out=out[e], accumulate=accumulate)
+        elif not accumulate:
+            out[e].zero_()
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
 # Embedding
 # ----------------------------------------------------------------------------------------------
 def embedding_fwd(tokens, w):

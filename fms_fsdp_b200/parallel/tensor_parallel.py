@@ -40,6 +40,9 @@ def refuse_unsupported_base(c):
     if getattr(c, "qk_norm", False) or getattr(c, "attn_head_dim", None) not in (None, c.emb_dim // c.nheads):
         raise NotImplementedError("speculator base models with QK-norm or a head_dim other than emb_dim / nheads "
                                   "(e.g. Qwen3) are not supported: the frozen-base attention path has no QK-norm")
+    if getattr(c, "moe_num_experts", 0) > 0:
+        raise NotImplementedError("mixture-of-experts Llama speculator bases are not supported: the frozen-base block "
+                                  "runs the dense feed-forward")
 
 
 def _check_llama_divisible(c, tp: int):

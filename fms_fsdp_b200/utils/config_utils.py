@@ -76,6 +76,15 @@ _LLAMA_ZOO: Dict[str, Dict[str, Any]] = {
     "qwen3_1.7b": _qwen3(2048, 6144, 28, 16),
     "qwen3_4b": _qwen3(2560, 9728, 36, 32),
     "qwen3_8b": _qwen3(4096, 12288, 36, 32),
+    # --- extensions: sparse mixture-of-experts checkpoints (every block's feed-forward is the MoE)
+    "qwen3_moe_30b_a3b": dict(_qwen3(2048, 6144, 48, 32), kvheads=4, moe_num_experts=128, moe_top_k=8,
+                              moe_hidden_dim=768, moe_norm_topk=True, moe_aux_loss_coef=0.001),
+    "mixtral_8x7b": dict(emb_dim=4096, nheads=32, kvheads=8, nlayers=32, max_expected_seq_len=32768,
+                         rope_theta=1000000.0, moe_num_experts=8, moe_top_k=2, moe_hidden_dim=14336,
+                         moe_norm_topk=True, moe_aux_loss_coef=0.02),
+    "llama_moe_tiny": dict(src_vocab_size=1024, emb_dim=256, nheads=4, kvheads=4, nlayers=2, max_expected_seq_len=512,
+                           moe_num_experts=8, moe_top_k=2, moe_hidden_dim=128, moe_norm_topk=True,
+                           moe_aux_loss_coef=0.01),
 }
 
 _MAMBA_ZOO: Dict[str, Dict[str, Any]] = {

@@ -16,7 +16,14 @@ The numbers follow what the runtime allocates (``parallel/engine.py``) and what 
   attention output, post-attention residual, gate|up and SwiGLU output = 2T(4D + 2*H*hd + 2*KV*hd + 3F) bytes, plus fp32
   row statistics; with QK-norm also the pre-norm q / k, 2T(H + KV)*hd bytes, and their rstd, 4T(H + KV) bytes; a
   recomputed block keeps its input only, one block's worth of activations is live while it is recomputed;
-* head: the final hidden states, their gradient and one [4096, V] logits chunk (+ its gradient in place).
+* head: the final hidden states, their gradient and one [4096, V] logits chunk (+ its gradient in place);
+* mixture of experts (``moe_num_experts`` E > 0, top-k, expert width F): the block's feed-forward parameters are the router
+  E*D and the experts 3*E*D*F.  ``ops.moe_mlp`` keeps, at the worst-case row count Mpad = round_up(T k + 127 E, 128) of
+  its expert-sorted buffer, the permuted input (Mpad*D), the gate|up projection (Mpad*2F), the SwiGLU output (Mpad*F) and
+  the expert outputs (Mpad*D) in bf16, the router probabilities (4 T E bytes), ids and weights (8 T k) and the int32
+  plan (4 (Mpad/128 + 2E + T k + Mpad)); its backward holds dY_perm, d(gate|up) and dX_perm (2 Mpad (2D + 2F) bytes)
+  for one block at a time, after the head's logits chunk and gradients are gone, so only the part of it beyond the
+  head's transient counts.
 
 Checked against the measured peak of the caching allocator: Llama2-1.4B, 1 H100 80GB HBM3 (400 W limit), seq 4096,
 batch 2, no recomputation = 31.19 GiB (``bench.py --gpus 1``), plan 31.18 GiB (``tests/test_config.py``).
@@ -66,19 +73,22 @@ def _recomputed_blocks(nlayers: int, selective_checkpointing, enabled: bool) -> 
 def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp", hsdp_shard_size: int = 0,
                batch_size: int = 2, seq_length: int = 4096, fsdp_activation_checkpointing: bool = False,
                selective_checkpointing="1", prefetch: int = 1, push_pool: int = 3, ce_chunk_rows: int = 4096,
-               grad_accum_steps: int = 1) -> MemoryPlan:
+               grad_accum_steps: int = 1, nlayers=None) -> MemoryPlan:
+    """``nlayers``: plan a stack truncated to that many blocks (None = the variant's depth)."""
     from fms_fsdp_b200.parallel.mesh import resolve_shard_size
     from fms_fsdp_b200.utils.config_utils import get_model_config
 
     c = get_model_config(model_variant)
-    D, F, V, L, hd = c.emb_dim, c.hidden_dim, c.src_vocab_size, c.nlayers, c.head_dim
+    D, F, V, L, hd = c.emb_dim, c.hidden_dim, c.src_vocab_size, nlayers or c.nlayers, c.head_dim
     kvd = c.kv_heads * hd
     S = resolve_shard_size(sharding_strategy, gpus, hsdp_shard_size, None)
     T = batch_size * seq_length
 
     qd = c.nheads * hd
     qk_norm = bool(getattr(c, "qk_norm", False))
-    block_params = (qd + 2 * kvd) * D + D * qd + 2 * F * D + D * F + 2 * D + (2 * hd if qk_norm else 0)
+    E, k, Fm = c.moe_num_experts, c.moe_top_k, c.moe_hidden_dim
+    ffn_params = E * D + 3 * E * D * Fm if E > 0 else 3 * F * D
+    block_params = (qd + 2 * kvd) * D + D * qd + ffn_params + 2 * D + (2 * hd if qk_norm else 0)
     root_params = 2 * V * D + D
     n_params = L * block_params + root_params
 
@@ -92,14 +102,24 @@ def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp
         parts[f"gathered parameters ({prefetch + 1} blocks + root, bf16)"] = 2.0 * ((prefetch + 1) * block_params + root_params) / GiB
         parts[f"gradient staging ({push_pool} block buffers + root, bf16)"] = 2.0 * (push_pool * block_params + root_params) / GiB
 
-    per_block = 2.0 * T * (4 * D + 2 * qd + 2 * kvd + 3 * F) + 4.0 * T * (2 + c.nheads)    # bf16 tensors + rstd x2 + lse
+    per_block = 2.0 * T * (4 * D + 2 * qd + 2 * kvd) + 4.0 * T * (2 + c.nheads)    # bf16 tensors + rstd x2 + lse
+    moe_bwd = 0.0
+    if E > 0:
+        Mpad = (T * k + 127 * E + 127) // 128 * 128
+        per_block += 2.0 * Mpad * (2 * D + 3 * Fm) + 4.0 * T * E + 8.0 * T * k + 4.0 * (Mpad // 128 + 2 * E + T * k + Mpad)
+        moe_bwd = 2.0 * Mpad * (2 * D + 2 * Fm)
+    else:
+        per_block += 2.0 * T * 3 * F
     if qk_norm:   # the QK-norm node also keeps the pre-norm q / k (bf16) and their per-head rstd (fp32)
         per_block += 2.0 * T * (qd + kvd) + 4.0 * T * (c.nheads + c.kv_heads)
     n_re = _recomputed_blocks(L, selective_checkpointing, fsdp_activation_checkpointing)
     kept = (L - n_re) * per_block + n_re * 2.0 * T * D + (per_block if n_re else 0.0)
     parts[f"activations ({L - n_re} blocks kept, {n_re} recomputed)"] = kept / GiB
     rows = min(ce_chunk_rows, T)
-    parts["head: hidden states + gradient + one logits chunk"] = (2 * 2.0 * T * D + 2.0 * rows * V + 2.0 * T * D) / GiB
+    head = 2 * 2.0 * T * D + 2.0 * rows * V + 2.0 * T * D
+    parts["head: hidden states + gradient + one logits chunk"] = head / GiB
+    if moe_bwd > head:
+        parts["MoE backward of one block beyond the head's transient"] = (moe_bwd - head) / GiB
     return MemoryPlan(model_variant, gpus, S, parts)
 
 

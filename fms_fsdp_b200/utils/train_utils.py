@@ -287,7 +287,12 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
     mcfg = getattr(getattr(model, "module", model), "config", None)
     flops_tok = None
     if mcfg is not None and hasattr(mcfg, "nlayers"):
-        flops_tok = model_flops_per_token(n_params, mcfg.nlayers, mcfg.emb_dim, cfg.seq_length)
+        # a mixture-of-experts model: only the router and k of E experts per block run for a token
+        n_active = n_params - (mcfg.inactive_params() if hasattr(mcfg, "inactive_params") else 0)
+        flops_tok = model_flops_per_token(n_active, mcfg.nlayers, mcfg.emb_dim, cfg.seq_length)
+    # MoE: the load-balancing loss of every micro-batch, summed on the device and read at report steps only
+    inner = getattr(model, "module", model)
+    moe_aux = torch.zeros((), device=device) if getattr(mcfg, "moe_num_experts", 0) > 0 else None
 
     ev0 = ev1 = None
     if is_cuda:
@@ -319,6 +324,8 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 micro_loss.backward()
                 micro_loss = micro_loss.detach()
             loss = micro_loss if loss is None else loss + micro_loss
+            if moe_aux is not None:
+                moe_aux += inner.moe_aux_loss().to(moe_aux.device)
         if accum > 1:
             loss = loss / accum
         gnorm = model.clip_grad_norm_(cfg.grad_clip_thresh)
@@ -352,6 +359,8 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 dev_step_time = t.item()
             if world_size > 1:
                 dist.all_reduce(ddp_stats, op=dist.ReduceOp.SUM)
+                if moe_aux is not None:
+                    dist.all_reduce(moe_aux, op=dist.ReduceOp.SUM)
             train_loss = ddp_stats[0] / ddp_stats[2]
             g_norm = ddp_stats[1] / ddp_stats[2]
             # failure detection the reference lacks (SURVEY.md 5.3): a non-finite loss / grad norm is surfaced at the
@@ -380,6 +389,8 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 print("LR:", current_lr)
                 print("tokens seen:", total_tokens_seen)
                 print("gradient norm:", current_gnorm)
+                if moe_aux is not None:   # coef * mean over layers, micro-batches, steps and ranks
+                    print("moe_aux_loss:", moe_aux.item() / (ddp_stats[2].item() * accum))
                 print("reserved memory:", reserved_mem)
                 print("allocated memory:", allocated_mem)
                 print("current step time:", current_step_time)
@@ -409,6 +420,8 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
             if is_cuda:
                 ev0.record()
             ddp_stats.zero_()
+            if moe_aux is not None:
+                moe_aux.zero_()
         if is_cuda:
             torch.cuda.reset_peak_memory_stats(device)
 

@@ -60,6 +60,12 @@ def main(**kwargs):
     if cfg.qk_norm:
         # per-head RMSNorm of q and k before RoPE (the qwen3_* variants have it already)
         llama_config.qk_norm = True
+    if llama_config.moe_num_experts > 0:
+        if cfg.precision == "fp8":
+            raise ValueError("--precision fp8 is not supported with a mixture-of-experts variant: the grouped expert "
+                             "GEMMs are bf16 only")
+        if cfg.moe_aux_loss_coef is not None:
+            llama_config.moe_aux_loss_coef = float(cfg.moe_aux_loss_coef)
     if cfg.low_cpu_fsdp or use_cuda:
         # one unit at a time is materialised directly on the device by the sharded runtime
         with torch.device("meta"):
