@@ -66,6 +66,9 @@ DECL int b200_sumsq(const void*, int, long long, float*, cudaStream_t);
 DECL int b200_attn_fwd(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t, const int*);
 DECL int b200_attn_bwd(const void*, const void*, const void*, const float*, void*, float*, int, int, int, int, int,
                        float, const float*, cudaStream_t, const int*);
+DECL int b200_attn_fwd_lockstep(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t, const int*);
+DECL int b200_attn_bwd_lockstep(const void*, const void*, const void*, const float*, void*, float*, int, int, int, int,
+                                int, float, const float*, cudaStream_t, const int*);
 DECL void b200_gemm2_set_rope(const float*, int, int, int);
 DECL void b200_gemm2_set_swiglu(void*, int, int, int);
 DECL void b200_gemm2_set_tile(int);
@@ -416,21 +419,24 @@ const int* seg_ptr(const c10::optional<at::Tensor>& seg, const at::Tensor& qkv, 
   return seg->data_ptr<int>();
 }
 
-std::vector<at::Tensor> attn_fwd(const at::Tensor& qkv, int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd,
-                                 double scale, const c10::optional<at::Tensor>& seg) {
+using AttnFwdFn = decltype(&b200_attn_fwd);
+using AttnBwdFn = decltype(&b200_attn_bwd);
+static std::vector<at::Tensor> attn_fwd_with(AttnFwdFn fn, const at::Tensor& qkv, int64_t B, int64_t S, int64_t H,
+                                             int64_t KVH, int64_t hd, double scale, const c10::optional<at::Tensor>& seg) {
   c10::cuda::CUDAGuard guard(qkv.device());
   need(qkv, "qkv", at::kBFloat16);
   TORCH_CHECK(qkv.is_contiguous());
   const int* seg_p = seg_ptr(seg, qkv, B, S);
   auto o = at::empty({B * S, H * hd}, qkv.options());
   auto lse = at::empty({B, H, S}, qkv.options().dtype(at::kFloat));
-  check(b200_attn_fwd(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, S, H, KVH, hd, (float)scale,
-                      cur_stream(), seg_p), "attn_fwd");
+  check(fn(qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), B, S, H, KVH, hd, (float)scale, cur_stream(), seg_p),
+        "attn_fwd");
   return {o, lse};
 }
-at::Tensor attn_bwd(const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o, const at::Tensor& lse,
-                    int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd, double scale,
-                    const c10::optional<at::Tensor>& rope, const c10::optional<at::Tensor>& seg) {
+static at::Tensor attn_bwd_with(AttnBwdFn fn, const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o,
+                                const at::Tensor& lse, int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd,
+                                double scale, const c10::optional<at::Tensor>& rope,
+                                const c10::optional<at::Tensor>& seg) {
   c10::cuda::CUDAGuard guard(qkv.device());
   need(qkv, "qkv", at::kBFloat16);
   need(dout, "do", at::kBFloat16);
@@ -447,10 +453,30 @@ at::Tensor attn_bwd(const at::Tensor& dout, const at::Tensor& qkv, const at::Ten
     TORCH_CHECK(rope->is_contiguous() && rope->numel() >= S * hd, "attn_bwd: rope table must be [S, hd/2, 2] fp32");
     rope_p = rope->data_ptr<float>();
   }
-  check(b200_attn_bwd(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
-                      delta.data_ptr<float>(), B, S, H, KVH, hd, (float)scale, rope_p, cur_stream(), seg_p),
+  check(fn(dout.data_ptr(), qkv.data_ptr(), o.data_ptr(), lse.data_ptr<float>(), dqkv.data_ptr(),
+           delta.data_ptr<float>(), B, S, H, KVH, hd, (float)scale, rope_p, cur_stream(), seg_p),
         "attn_bwd", 3);
   return dqkv;
+}
+std::vector<at::Tensor> attn_fwd(const at::Tensor& qkv, int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd,
+                                 double scale, const c10::optional<at::Tensor>& seg) {
+  return attn_fwd_with(b200_attn_fwd, qkv, B, S, H, KVH, hd, scale, seg);
+}
+at::Tensor attn_bwd(const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o, const at::Tensor& lse,
+                    int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd, double scale,
+                    const c10::optional<at::Tensor>& rope, const c10::optional<at::Tensor>& seg) {
+  return attn_bwd_with(b200_attn_bwd, dout, qkv, o, lse, B, S, H, KVH, hd, scale, rope, seg);
+}
+// the lock-step attention kernels: bitwise the same outputs, kept as the reference the pipelined kernels are checked
+// and timed against (tests, scripts/attn_bench.py)
+std::vector<at::Tensor> attn_fwd_lockstep(const at::Tensor& qkv, int64_t B, int64_t S, int64_t H, int64_t KVH,
+                                          int64_t hd, double scale, const c10::optional<at::Tensor>& seg) {
+  return attn_fwd_with(b200_attn_fwd_lockstep, qkv, B, S, H, KVH, hd, scale, seg);
+}
+at::Tensor attn_bwd_lockstep(const at::Tensor& dout, const at::Tensor& qkv, const at::Tensor& o, const at::Tensor& lse,
+                             int64_t B, int64_t S, int64_t H, int64_t KVH, int64_t hd, double scale,
+                             const c10::optional<at::Tensor>& rope, const c10::optional<at::Tensor>& seg) {
+  return attn_bwd_with(b200_attn_bwd_lockstep, dout, qkv, o, lse, B, S, H, KVH, hd, scale, rope, seg);
 }
 
 // ---- peer-memory collectives: pointer tables live on the device (int64 tensors of peer addresses)
@@ -1028,6 +1054,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("attn_bwd", &attn_bwd, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"), py::arg("B"), py::arg("S"),
         py::arg("H"), py::arg("KVH"), py::arg("hd"), py::arg("scale"), py::arg("rope") = py::none(),
         py::arg("seg") = py::none());
+  m.def("attn_fwd_lockstep", &attn_fwd_lockstep, py::arg("qkv"), py::arg("B"), py::arg("S"), py::arg("H"),
+        py::arg("KVH"), py::arg("hd"), py::arg("scale"), py::arg("seg") = py::none());
+  m.def("attn_bwd_lockstep", &attn_bwd_lockstep, py::arg("dout"), py::arg("qkv"), py::arg("o"), py::arg("lse"),
+        py::arg("B"), py::arg("S"), py::arg("H"), py::arg("KVH"), py::arg("hd"), py::arg("scale"),
+        py::arg("rope") = py::none(), py::arg("seg") = py::none());
   m.def("p2p_allgather", &p2p_allgather);
   m.def("reduce_scatter", &reduce_scatter, py::arg("peer_ptrs"), py::arg("out32"), py::arg("elem_offset"), py::arg("world"),
         py::arg("rank"), py::arg("src_bf16"), py::arg("scale"), py::arg("sumsq_out"), py::arg("max_ctas") = 0,
