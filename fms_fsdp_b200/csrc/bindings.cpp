@@ -69,7 +69,9 @@ DECL int b200_attn_bwd(const void*, const void*, const void*, const float*, void
 DECL int b200_attn_fwd_lockstep(const void*, void*, float*, int, int, int, int, int, float, cudaStream_t, const int*);
 DECL int b200_attn_bwd_lockstep(const void*, const void*, const void*, const float*, void*, float*, int, int, int, int,
                                 int, float, const float*, cudaStream_t, const int*);
-DECL void b200_gemm2_set_rope(const float*, int, int, int);
+DECL int b200_bias_grad_slices(int, int);
+DECL int b200_bias_grad(const void*, float*, float*, int, int, int, cudaStream_t);
+DECL void b200_gemm2_set_rope(const float*, int, int, int, const void*);
 DECL void b200_gemm2_set_swiglu(void*, int, int, int);
 DECL void b200_gemm2_set_tile(int);
 DECL int b200_gemm2_fp8(const void*, const void*, void*, const float*, const float*, int, int, int, int, int, int, cudaStream_t);
@@ -105,6 +107,7 @@ namespace {
 static int64_t g_launches = 0;
 static int g_reduce_ctas_default = 264;  // 2 CTAs per SM of an H100
 static bool g_gemm_2cta = true;
+static int64_t g_rope_bias_n = -1;        // length of the bias of the next RoPE-bias GEMM (-1: none set)
 
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
@@ -157,8 +160,9 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layou
     r = residual->data_ptr();
     ldr = residual->stride(0);
   }
-  TORCH_CHECK(epi != 3 || (g_gemm_2cta && M >= 256 && layout == 0 && c.scalar_type() == at::kBFloat16),
+  TORCH_CHECK((epi != 3 && epi != 8) || (g_gemm_2cta && M >= 256 && layout == 0 && c.scalar_type() == at::kBFloat16),
               "RoPE epilogue: M >= 256, nt layout, bf16 output only (call set_gemm_rope first)");
+  TORCH_CHECK(epi != 8 || g_rope_bias_n == N, "RoPE-bias epilogue: set_gemm_rope(..., bias) with a [N] bias first");
   TORCH_CHECK(epi != 4, "push epilogue: use gemm_push (no output tensor)");
   // fused-epilogue entry for anything with at least 256 rows; the store / residual / accumulate entry otherwise
   if (g_gemm_2cta && M >= 256) {
@@ -318,6 +322,19 @@ std::vector<at::Tensor> qk_norm_bwd(at::Tensor& dqkv, const at::Tensor& xqk, con
                          part.data_ptr<float>(), dw.data_ptr<float>(), M, dqkv.stride(0), (int)H, (int)KVH, (int)hd,
                          cur_stream()), "qk_norm_bwd", 2);
   return {dw[0], dw[1]};
+}
+// fp32 db[n] = sum_t dy[t, n] of a projection's output gradient dy [T, N] (bf16), reduced in a fixed order
+at::Tensor bias_grad(const at::Tensor& dy) {
+  c10::cuda::CUDAGuard guard(dy.device());
+  need(dy, "dy", at::kBFloat16);
+  need_rowmajor2d(dy, "dy");
+  const int T = dy.size(0), N = dy.size(1);
+  TORCH_CHECK(T > 0 && N % 8 == 0, "bias_grad: needs rows and a width that is a multiple of 8");
+  auto part = at::empty({b200_bias_grad_slices(T, N), N}, dy.options().dtype(at::kFloat));
+  auto db = at::empty({N}, dy.options().dtype(at::kFloat));
+  check(b200_bias_grad(dy.data_ptr(), part.data_ptr<float>(), db.data_ptr<float>(), T, N, (int)dy.stride(0), cur_stream()),
+        "bias_grad", 2);
+  return db;
 }
 at::Tensor swiglu_fwd(const at::Tensor& gu, bool gate_first) {
   c10::cuda::CUDAGuard guard(gu.device());
@@ -579,6 +596,7 @@ void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::T
   else if (layout == 1) { M = a.size(0); K = a.size(1); N = b.size(1); b_mn = 1; TORCH_CHECK(b.size(0) == K); }
   else { K = a.size(0); M = a.size(1); N = b.size(1); a_mn = b_mn = 1; TORCH_CHECK(b.size(0) == K); }
   TORCH_CHECK(c.size(0) == M && c.size(1) == (epi == 6 ? 2 * N : N) && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0);
+  TORCH_CHECK(epi != 8 || g_rope_bias_n == N, "RoPE-bias epilogue: set_gemm_rope(..., bias) with a [N] bias first");
   const void* r = nullptr;
   int ldr = 0;
   if (epi == 1) {
@@ -1041,6 +1059,7 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rope", &rope);
   m.def("qk_norm_rope", &qk_norm_rope);
   m.def("qk_norm_bwd", &qk_norm_bwd);
+  m.def("bias_grad", &bias_grad);
   m.def("swiglu_fwd", &swiglu_fwd);
   m.def("swiglu_bwd", &swiglu_bwd);
   m.def("embedding_fwd", &embedding_fwd);
@@ -1071,11 +1090,22 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("causal_conv1d_fwd", &causal_conv1d_fwd);
   m.def("causal_conv1d_bwd", &causal_conv1d_bwd);
   m.def("set_reduce_ctas", [](int64_t n) { g_reduce_ctas_default = n < 1 ? 1 : (int)n; b200_comm_set_reduce_ctas((int)n); });
-  m.def("set_gemm_rope", [](const at::Tensor& table, int64_t S, int64_t hd, int64_t cols) {
+  m.def("set_gemm_rope", [](const at::Tensor& table, int64_t S, int64_t hd, int64_t cols,
+                            const c10::optional<at::Tensor>& bias) {
+    // bias: the [N] bf16 q / k / v bias the next RoPE-bias GEMM (epi 8) adds before the rotation
     need(table, "rope table", at::kFloat);
     TORCH_CHECK(table.is_contiguous() && table.numel() >= S * hd, "rope table must be [S, hd/2, 2] fp32");
-    b200_gemm2_set_rope(table.data_ptr<float>(), (int)S, (int)hd, (int)cols);
-  });
+    const void* b = nullptr;
+    g_rope_bias_n = -1;
+    if (bias.has_value() && bias->defined()) {
+      need(*bias, "qkv bias", at::kBFloat16);
+      TORCH_CHECK(bias->dim() == 1 && bias->is_contiguous() && (reinterpret_cast<uintptr_t>(bias->data_ptr()) & 3) == 0,
+                  "qkv bias must be a contiguous, 4-byte aligned [N] vector");
+      b = bias->data_ptr();
+      g_rope_bias_n = bias->numel();
+    }
+    b200_gemm2_set_rope(table.data_ptr<float>(), (int)S, (int)hd, (int)cols, b);
+  }, py::arg("table"), py::arg("S"), py::arg("hd"), py::arg("cols"), py::arg("bias") = py::none());
   m.def("push_range", [](const at::Tensor& src, const at::Tensor& bases, int64_t n, int64_t off, int64_t rank) {
     // this rank's gradient elements [off, off + src.numel()) -> the owners' staging slots (norm gains / biases)
     c10::cuda::CUDAGuard guard(src.device());

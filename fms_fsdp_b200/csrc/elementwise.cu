@@ -840,6 +840,50 @@ __global__ void __launch_bounds__(256) qk_norm_bwd_kernel(__nv_bfloat16* __restr
   }
 }
 
+// Gradient of a projection bias, pass 1: part[slice][n] = sum over the rows of one row slice of dy[t, n] (fp32).  A CTA
+// covers 256 columns of one slice: lane l holds columns 8 l .. 8 l + 7 (one 16-byte load per row), warp w the rows
+// r0 + w, r0 + w + 8, ...; the 8 warps are then folded in warp order.  colsum_kernel sums the slices in order: no float
+// atomics, the bits depend on the shape only.
+__global__ void __launch_bounds__(256) bias_grad_kernel(const __nv_bfloat16* __restrict__ dy, float* __restrict__ part,
+                                                        int T, int N, int ld, int rows_per_slice) {
+  __shared__ __align__(16) float sh[8][256];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int col = blockIdx.x * 256 + lane * 8;
+  const int r0 = blockIdx.y * rows_per_slice, r1 = min(T, r0 + rows_per_slice);
+  float acc[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) acc[i] = 0.f;
+  if (col < N) {
+    int r = r0 + warp;
+    for (; r + 24 < r1; r += 32) {                 // four rows in flight per warp
+      float v[4][8];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) load8(dy + (size_t)(r + 8 * u) * ld + col, v[u]);
+#pragma unroll
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) acc[i] += v[u][i];
+    }
+    for (; r < r1; r += 8) {
+      float v[8];
+      load8(dy + (size_t)r * ld + col, v);
+#pragma unroll
+      for (int i = 0; i < 8; ++i) acc[i] += v[i];
+    }
+  }
+  float4* s = reinterpret_cast<float4*>(&sh[warp][lane * 8]);
+  s[0] = make_float4(acc[0], acc[1], acc[2], acc[3]);
+  s[1] = make_float4(acc[4], acc[5], acc[6], acc[7]);
+  __syncthreads();
+  const int c = blockIdx.x * 256 + threadIdx.x;
+  if (c < N) {
+    float t = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) t += sh[w][threadIdx.x];
+    part[(size_t)blockIdx.y * N + c] = t;
+  }
+}
+
 static inline int grid_for(size_t work_items, int threads, int max_blocks = 132 * 8) {
   size_t b = (work_items + threads - 1) / threads;
   if (b < 1) b = 1;
@@ -1030,6 +1074,30 @@ extern "C" int b200_qk_norm_bwd(void* dqkv, const void* xqk, const float* rstd, 
   if (hd == 64) B200_QKN_BWD(64); else B200_QKN_BWD(128);
 #undef B200_QKN_BWD
   colsum_kernel<<<(2 * hd + 31) / 32, 256, 0, s>>>(dw_part, dw, grid, 2 * hd);
+  CK();
+}
+// Row slices of bias_grad: about 4 CTAs per SM of an H100 over all column blocks, at least 32 rows each.  Fixed for a
+// given shape (the reduction order, and so the bits, depend on it).
+static void bias_grad_slices(int T, int N, int* slices, int* rows) {
+  const int col_blocks = (N + 255) / 256;
+  int p = (132 * 4) / col_blocks;
+  if (p > (T + 31) / 32) p = (T + 31) / 32;
+  if (p < 1) p = 1;
+  *rows = (T + p - 1) / p;
+  *slices = (T + *rows - 1) / *rows;
+}
+extern "C" int b200_bias_grad_slices(int T, int N) {
+  int slices, rows;
+  bias_grad_slices(T, N, &slices, &rows);
+  return slices;
+}
+// db[n] = sum_t dy[t, n] (fp32) over dy [T, N] bf16 (row stride ld); part: [b200_bias_grad_slices(T, N), N] fp32
+extern "C" int b200_bias_grad(const void* dy, float* part, float* db, int T, int N, int ld, cudaStream_t s) {
+  if (T <= 0 || N % 8 || ld % 8 || (reinterpret_cast<uintptr_t>(dy) & 15)) return -1;
+  int slices, rows;
+  bias_grad_slices(T, N, &slices, &rows);
+  bias_grad_kernel<<<dim3((N + 255) / 256, slices), 256, 0, s>>>((const __nv_bfloat16*)dy, part, T, N, ld, rows);
+  colsum_kernel<<<(N + 31) / 32, 256, 0, s>>>(part, db, slices, N);
   CK();
 }
 

@@ -8,7 +8,8 @@
 //   dgrad    dx = dy W   : A K-major [M,Nr], B MN-major (W is [Nr,K])   ("nn")
 //   wgrad    dW = dy^T x : A MN-major (dy is [Mr,N]), B MN-major        ("tn")
 // The MN-major cases use wgmma's transposed-operand smem layout, so no transposes are ever materialised.
-// Epilogues: plain store, +residual, accumulate into C, RoPE on the QKV projection, SwiGLU (forward and backward),
+// Epilogues: plain store, +residual, accumulate into C, RoPE on the QKV projection (optionally after adding its bias),
+// SwiGLU (forward and backward),
 // push of wgrad tiles to the owning rank, per-row/column scales of the e4m3 path; bf16 or fp32 output.
 //
 // Warp roles (384 threads): warpgroup 0 = producer (warp 0 lane 0 issues TMA; warps 2-3 are the comm warps of the fused
@@ -41,7 +42,7 @@ __host__ __device__ constexpr int smem_bytes() {   // ring + 1 KiB alignment sla
 }
 
 enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_ACCUM = 2, EPI_ROPE = 3, EPI_PUSH = 4, EPI_SWIGLU = 5, EPI_SWIGLU_BWD = 6,
-       EPI_SCALE = 7 };
+       EPI_SCALE = 7, EPI_ROPE_BIAS = 8 };
 // Grouped (mixture-of-experts) launches of the 128 x 128 kernel carry their mode in the high bits of the EPI template
 // argument, so the instantiations that existed before them keep their names and their code.  Operands live in the
 // expert-sorted row buffer of csrc/moe.cu; the expert weights are one tensor whose rows hold all experts.
@@ -155,8 +156,10 @@ struct GemmParams {
   int ld_aux, swi_F, swi_gate_first;
   // EPI_SCALE (fp8 e4m3 operands, FP8 = true): C = acc * scale_a[row] * scale_b[col].  GRP_K: grp_seg = the plan's
   // [start | len] of every expert.
+  // EPI_ROPE_BIAS (QKV projection with q / k / v biases): bias [N] bf16 is added to the accumulator, then the q / k
+  // columns are rotated as in EPI_ROPE.  fp8 launches never rotate, so the bias shares scale_b's slot.
   union { const float* scale_a; const int* grp_seg; };
-  const float* scale_b;
+  union { const float* scale_b; const __nv_bfloat16* bias; };
 };
 
 B200_DEVINL void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
@@ -195,7 +198,11 @@ B200_DEVINL void epi_pair(const GemmParams& p, OutT* crow, int row, int col, flo
     const float sa = p.scale_a[row];
     const float2 sb = *reinterpret_cast<const float2*>(p.scale_b + col);
     f0 *= sa * sb.x; f1 *= sa * sb.y;
-  } else if constexpr (EPI == EPI_ROPE) {
+  } else if constexpr (EPI == EPI_ROPE || EPI == EPI_ROPE_BIAS) {
+    if constexpr (EPI == EPI_ROPE_BIAS) {
+      const float2 b = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p.bias + col));
+      f0 += b.x; f1 += b.y;
+    }
     if (col < p.rope_cols) {
       const float2 cs = *reinterpret_cast<const float2*>(
           p.rope + ((size_t)(row % p.rope_S) * (p.rope_hd >> 1) + ((col % p.rope_hd) >> 1)) * 2);
@@ -529,7 +536,8 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
 // warpgroup issues m64n256k16, which reads 10 KiB of shared-memory operands per 524k FLOP where two m64n128k16 read
 // 12 KiB.  A 64 x 256 fp32 accumulator is 128 registers per consumer thread, more than 384 threads get by default:
 // setmaxnreg hands the producer warpgroup's registers to the consumers (128 x 40 + 256 x 232 <= 64K).
-// Epilogues: store, +residual, accumulate (bf16 or fp32 output), RoPE, SwiGLU forward (F % 128 == 0) and backward.
+// Epilogues: store, +residual, accumulate (bf16 or fp32 output), RoPE (with or without bias), SwiGLU forward
+// (F % 128 == 0) and backward.
 constexpr int WBN = 256;
 constexpr int W_STAGES = 4;
 constexpr int W_STAGE_BYTES = A_BYTES + WBN * BK * 2;   // 16 + 32 KiB
@@ -729,9 +737,10 @@ static int make_maps(CUtensorMap* tmA, CUtensorMap* tmB, const void* A, const vo
   return 0;
 }
 
-// RoPE epilogue parameters of the NEXT epi == EPI_ROPE launch (set immediately before it by the single host thread
-// that owns the stream; keeps the launcher signatures unchanged)
+// RoPE epilogue parameters of the NEXT epi == EPI_ROPE / EPI_ROPE_BIAS launch (set immediately before it by the single
+// host thread that owns the stream; keeps the launcher signatures unchanged)
 static const float* g_rope_table = nullptr;
+static const __nv_bfloat16* g_rope_bias = nullptr;
 static int g_rope_S = 1, g_rope_hd = 2, g_rope_cols = 0;
 // same convention for the push epilogue
 static void* const* g_push_bases = nullptr;
@@ -751,6 +760,7 @@ static GemmParams make_params(void* C, const void* R, int M, int N, int K, int l
   p.push_bases = g_push_bases; p.push_n = g_push_n; p.push_off = g_push_off; p.push_rank = g_push_rank;
   p.push_bulk = g_push_bulk;
   p.aux = g_swi_aux; p.ld_aux = g_swi_ld; p.swi_F = g_swi_F; p.swi_gate_first = g_swi_gate_first;
+  if (epi == EPI_ROPE_BIAS) p.bias = g_rope_bias;
   if (epi == EPI_PUSH && g_push_world > 1) {
     const int per_band = GROUP_M * p.n_tiles, tiles = p.m_tiles * p.n_tiles;
     const int bands = (tiles + per_band - 1) / per_band;
@@ -761,8 +771,10 @@ static GemmParams make_params(void* C, const void* R, int M, int N, int K, int l
 
 }  // namespace b200
 
-extern "C" void b200_gemm2_set_rope(const float* table, int S, int hd, int cols) {
+// bias: [N] bf16, 4-byte aligned, read by EPI_ROPE_BIAS launches only (nullptr otherwise)
+extern "C" void b200_gemm2_set_rope(const float* table, int S, int hd, int cols, const void* bias) {
   b200::g_rope_table = table; b200::g_rope_S = S; b200::g_rope_hd = hd; b200::g_rope_cols = cols;
+  b200::g_rope_bias = static_cast<const __nv_bfloat16*>(bias);
 }
 
 // world > 1: rotate the tile raster by rank * tiles / world (0 / 1 = no rotation).  bulk = 1: tiles are staged in shared
@@ -799,9 +811,11 @@ extern "C" int b200_gemm2_bf16(const void* A, const void* B, void* C, const void
     if (a_mn || !b_mn || out_fp32 || !p.aux || p.swi_F != N || (N % 8) || (p.ld_aux % 8)) return -12;
     return launch_local<false, true, EPI_SWIGLU_BWD, __nv_bfloat16>(tmA, tmB, p, stream);
   }
-  if (epi == EPI_ROPE) {
+  if (epi == EPI_ROPE || epi == EPI_ROPE_BIAS) {
     if (a_mn || b_mn || out_fp32 || !p.rope || (p.rope_hd % 8) || (p.rope_cols % 8)) return -8;
-    return launch_local<false, false, EPI_ROPE, __nv_bfloat16>(tmA, tmB, p, stream);
+    if (epi == EPI_ROPE) return launch_local<false, false, EPI_ROPE, __nv_bfloat16>(tmA, tmB, p, stream);
+    if (!p.bias) return -8;
+    return launch_local<false, false, EPI_ROPE_BIAS, __nv_bfloat16>(tmA, tmB, p, stream);
   }
   if (epi == EPI_PUSH) {   // wgrad (tn) only; every 8-element vector must stay inside one owner's slice
     if (!a_mn || !b_mn || out_fp32 || !p.push_bases || p.push_n <= 0 || (p.push_n % 8) || (p.push_off % 8) || (ldc % 8))
@@ -911,7 +925,7 @@ extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, con
   return launch<false, true, G | EPI_STORE, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
 }
 
-// GEMM + fused all-gather.  Supported: bf16 output, EPI store|residual|rope|swiglu (nt), store|residual|swiglu_bwd (nn),
+// GEMM + fused all-gather.  Supported: bf16 output, EPI store|residual|rope|rope_bias|swiglu (nt), store|residual|swiglu_bwd (nn),
 // store|accumulate|push (tn).
 extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda,
                                   int ldb, int ldc, int ldr, int a_mn, int b_mn, int epi,
@@ -936,9 +950,11 @@ extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const v
   ag.b_row_bytes = (unsigned long long)ldb * 2;
   if (dependent && ((const uint8_t*)B < (const uint8_t*)full)) return -6;
 #define AGL(AM, BM_, E) return launch<AM, BM_, E, __nv_bfloat16, true>(tmA, tmB, p, ag, stream)
-  if (epi == EPI_ROPE) {
+  if (epi == EPI_ROPE || epi == EPI_ROPE_BIAS) {
     if (a_mn || b_mn || !p.rope || (p.rope_hd % 8) || (p.rope_cols % 8)) return -8;
-    AGL(false, false, EPI_ROPE);
+    if (epi == EPI_ROPE) AGL(false, false, EPI_ROPE);
+    if (!p.bias) return -8;
+    AGL(false, false, EPI_ROPE_BIAS);
   }
   if (!a_mn && !b_mn) {
     if (epi == EPI_SWIGLU) AGL(false, false, EPI_SWIGLU);

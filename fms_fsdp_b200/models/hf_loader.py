@@ -6,6 +6,8 @@ the adapters of ``train_speculator_utils.py:526-569``):
   to the FMS interleaved-pair layout (the inverse of ``fms_to_hf_llama._interleaved_to_halfsplit``);
 * Qwen3 (dense) -> ``LLaMA`` with ``qk_norm`` and an explicit head dim: as Llama, plus the per-head ``q_norm`` / ``k_norm``
   gains permuted the same way as the q / k rows (tied embeddings are read as an untied copy);
+* Qwen2 / Qwen2.5 -> ``LLaMA`` with ``qkv_bias``: as Llama, plus the q / k / v biases fused like the weights, the q / k
+  biases permuted head by head like their rows (tied embeddings are read as an untied copy);
 * GPT-BigCode (multi-query attention, learned positions) -> ``EmbedGPTBigCode``;
 * Mixtral (Llama attention + top-k sparse MoE) -> ``EmbedMixtral``; both the hub format (``block_sparse_moe.experts.N.w1/w2/w3``)
   and the fused in-memory format of recent transformers (``mlp.experts.gate_up_proj / down_proj``)."""
@@ -31,11 +33,19 @@ def _halfsplit_to_interleaved_vec(w: torch.Tensor) -> torch.Tensor:
     return _halfsplit_to_interleaved(w.view(-1, 1), 1).view(-1)
 
 
+def _halfsplit_to_interleaved_bias(b: torch.Tensor, nheads: int) -> torch.Tensor:
+    """A q or k projection bias [nheads * hd] in the order of the permuted rows: each head's entries move like that
+    head's rows (``_halfsplit_to_interleaved_vec`` would treat the whole bias as one head)."""
+    return _halfsplit_to_interleaved(b.view(-1, 1), nheads).view(-1)
+
+
 # model types whose differences from the Llama block are not implemented here (loading them would change the logits)
 _REFUSED_MODEL_TYPES = {
     "olmo2": "q / k RMSNorm over the whole projection instead of per head",
     "olmo3": "q / k RMSNorm over the whole projection instead of per head",
-    "qwen2": "q / k / v projection biases",
+    # Qwen2 is loaded when the checkpoint's tensors are at hand and show q / k / v biases without an output bias
+    # (config_from_hf with ``tensors``); the config alone cannot show it
+    "qwen2": "q / k / v projection biases; pass the checkpoint's tensors to detect them",
     # the engine trains these feed-forwards (LLaMAConfig.moe_num_experts) but does not import their checkpoints yet;
     # Mixtral is refused by convert_hf_state_dict instead (its attention config also serves the frozen speculator base)
     "qwen3_moe": "sparse mixture-of-experts feed-forward",
@@ -43,12 +53,24 @@ _REFUSED_MODEL_TYPES = {
 }
 
 
-def _refuse_unsupported(hf_cfg: dict):
-    """Features this repo's models do not implement must stop the load instead of silently changing the logits."""
+def _has_qkv_bias_only(hf_cfg: dict, tensors: Optional[Dict[str, torch.Tensor]]) -> bool:
+    """The checkpoint's tensors show Qwen2 attention: every layer biases q, k and v, and no layer biases o_proj."""
+    if tensors is None:
+        return False
+    for i in range(hf_cfg["num_hidden_layers"]):
+        s = f"model.layers.{i}.self_attn."
+        if not all(s + f"{n}_proj.bias" in tensors for n in "qkv") or s + "o_proj.bias" in tensors:
+            return False
+    return True
+
+
+def _refuse_unsupported(hf_cfg: dict, qkv_bias: bool = False):
+    """Features this repo's models do not implement must stop the load instead of silently changing the logits.
+    ``qkv_bias``: the tensors showed Qwen2's q / k / v biases, which are implemented (``LLaMAConfig.qkv_bias``)."""
     why = _REFUSED_MODEL_TYPES.get(hf_cfg.get("model_type"))
-    if why:
-        raise NotImplementedError(f"HF model type {hf_cfg['model_type']!r} is not supported ({why}); Llama and Qwen3 dense "
-                                  "checkpoints are")
+    if why and not (qkv_bias and hf_cfg.get("model_type") == "qwen2"):
+        raise NotImplementedError(f"HF model type {hf_cfg['model_type']!r} is not supported ({why}); Llama, Qwen2 / Qwen2.5 "
+                                  "and Qwen3 dense checkpoints are")
     scaling = hf_cfg.get("rope_scaling") or {}
     params = hf_cfg.get("rope_parameters") or {}
     kind = scaling.get("rope_type") or scaling.get("type") or params.get("rope_type") or "default"
@@ -60,7 +82,8 @@ def _refuse_unsupported(hf_cfg: dict):
         raise NotImplementedError(f"HF checkpoint uses sliding-window attention (window {window}); only full causal attention is "
                                   "implemented")
     if hf_cfg.get("attention_bias") or hf_cfg.get("mlp_bias"):
-        raise NotImplementedError("HF checkpoint has attention / MLP biases; the LLaMA blocks here are bias-free")
+        raise NotImplementedError("HF checkpoint has attention / MLP biases; the LLaMA blocks here have q / k / v "
+                                  "biases only (Qwen2), no output or MLP biases")
 
 
 _Q_NORM_KEY = "model.layers.0.self_attn.q_norm.weight"
@@ -68,8 +91,10 @@ _Q_NORM_KEY = "model.layers.0.self_attn.q_norm.weight"
 
 def config_from_hf(hf_cfg: dict, tensors: Optional[Dict[str, torch.Tensor]] = None) -> LLaMAConfig:
     """``tensors`` (optional): the checkpoint's tensors; a per-head ``self_attn.q_norm.weight`` there turns QK-norm on
-    whatever ``model_type`` says."""
-    _refuse_unsupported(hf_cfg)
+    whatever ``model_type`` says, and q / k / v biases in every layer without an output bias (Qwen2) turn on
+    ``qkv_bias``.  Without them a ``qwen2`` config is refused."""
+    qkv_bias = hf_cfg.get("model_type") == "qwen2" and _has_qkv_bias_only(hf_cfg, tensors)
+    _refuse_unsupported(hf_cfg, qkv_bias)
     D, F = hf_cfg["hidden_size"], hf_cfg["intermediate_size"]
     H = hf_cfg["num_attention_heads"]
     hd = hf_cfg.get("head_dim") or D // H
@@ -88,7 +113,7 @@ def config_from_hf(hf_cfg: dict, tensors: Optional[Dict[str, torch.Tensor]] = No
         nheads=H, kvheads=hf_cfg.get("num_key_value_heads", 0) or 0,
         nlayers=hf_cfg["num_hidden_layers"], hidden_grow_factor=F / D, multiple_of=1,
         max_expected_seq_len=hf_cfg.get("max_position_embeddings", 4096), rope_theta=float(rope),
-        rope_scaling=rope_scaling, qk_norm=qk_norm, attn_head_dim=hd if hd != D // H else None)
+        rope_scaling=rope_scaling, qk_norm=qk_norm, attn_head_dim=hd if hd != D // H else None, qkv_bias=qkv_bias)
 
 
 def _read_hf_tensors(model_path: str) -> Dict[str, torch.Tensor]:
@@ -118,6 +143,13 @@ def convert_hf_state_dict(hf: Dict[str, torch.Tensor], cfg: LLaMAConfig) -> Dict
         q = _halfsplit_to_interleaved(hf[s + "self_attn.q_proj.weight"], cfg.nheads)
         k = _halfsplit_to_interleaved(hf[s + "self_attn.k_proj.weight"], cfg.kv_heads)
         sd[d + "attn.in_proj.qkv_fused.weight"] = torch.cat([q, k, hf[s + "self_attn.v_proj.weight"]], dim=0)
+        if (s + "self_attn.q_proj.bias" in hf) != bool(cfg.qkv_bias):
+            raise ValueError(f"layer {i}: the checkpoint {'lacks' if cfg.qkv_bias else 'has'} q / k / v biases "
+                             f"but the config says qkv_bias={cfg.qkv_bias}")
+        if cfg.qkv_bias:   # the q / k biases follow their rows from half-split to interleaved order, head by head
+            qb = _halfsplit_to_interleaved_bias(hf[s + "self_attn.q_proj.bias"], cfg.nheads)
+            kb = _halfsplit_to_interleaved_bias(hf[s + "self_attn.k_proj.bias"], cfg.kv_heads)
+            sd[d + "attn.in_proj.qkv_fused.bias"] = torch.cat([qb, kb, hf[s + "self_attn.v_proj.bias"]])
         sd[d + "attn.dense.weight"] = hf[s + "self_attn.o_proj.weight"]
         sd[d + "ff_sub_layer.wg1_fused.weight"] = torch.cat([hf[s + "mlp.gate_proj.weight"], hf[s + "mlp.up_proj.weight"]], dim=0)
         sd[d + "ff_sub_layer.w2.weight"] = hf[s + "mlp.down_proj.weight"]

@@ -57,6 +57,10 @@ class LLaMAConfig:
     # extension (not an fms field): head dimension when it is not emb_dim // nheads (Qwen3-0.6B / 4B: 128 with
     # emb_dim / nheads = 64 / 80).  None = emb_dim // nheads.
     attn_head_dim: Optional[int] = None
+    # extension (not an fms field): q / k / v projection biases (Qwen2 / Qwen2.5) -- ``attn.in_proj.qkv_fused.bias``
+    # [(nheads + 2 kv_heads) * head_dim], added before RoPE.  Unlike fms's ``attn_bias`` the output projection stays
+    # bias-free.
+    qkv_bias: bool = False
     # extension (not an fms field): sparse mixture-of-experts feed-forward (Qwen3-MoE, Mixtral).  moe_num_experts > 0
     # replaces every block's ``ff_sub_layer`` with ``moe``: router ``moe.gate.weight`` [E, D] and SwiGLU experts
     # ``moe.w1`` [E, 2F, D] ([gate | up] per expert) and ``moe.w2`` [E, D, F], F = moe_hidden_dim.  Each token goes to
@@ -158,6 +162,8 @@ class _InProj(nn.Module):
         hd = cfg.head_dim
         self.splits = [cfg.nheads * hd, cfg.kv_heads * hd, cfg.kv_heads * hd]
         self.qkv_fused = _Weight(sum(self.splits), cfg.emb_dim, device, dtype)
+        if cfg.qkv_bias:   # q / k sections in the interleaved RoPE pair order of the weight's rows
+            self.qkv_fused.bias = nn.Parameter(torch.empty(sum(self.splits), device=device, dtype=dtype))
 
 
 class MultiHeadAttention(nn.Module):
@@ -171,6 +177,7 @@ class MultiHeadAttention(nn.Module):
         if self.qk_norm:   # per-head gains, indexed by position within a head (interleaved RoPE pair order)
             self.q_norm = RMSNorm(cfg.head_dim, cfg.norm_eps, device, dtype)
             self.k_norm = RMSNorm(cfg.head_dim, cfg.norm_eps, device, dtype)
+        self.qkv_bias = bool(cfg.qkv_bias)
 
     def reset_parameters(self):
         for w in (self.in_proj.qkv_fused.weight, self.dense.weight):
@@ -178,10 +185,16 @@ class MultiHeadAttention(nn.Module):
         if self.qk_norm:
             self.q_norm.reset_parameters()
             self.k_norm.reset_parameters()
+        if self.qkv_bias:
+            nn.init.zeros_(self.in_proj.qkv_fused.bias)
 
     def qk_norm_args(self):
         """``ops.qkv_attention(qk_norm=...)``: None without QK-norm."""
         return (self.q_norm.weight, self.k_norm.weight, self.q_norm.eps) if self.qk_norm else None
+
+    def qkv_bias_arg(self):
+        """``ops.qkv_attention(qkv_bias=...)``: None without projection biases."""
+        return self.in_proj.qkv_fused.bias if self.qkv_bias else None
 
 
 class GatedLinearUnit(nn.Module):
@@ -271,7 +284,7 @@ class LLaMABlock(nn.Module):
         h, x = self.ln.fork(x)
         # projection + RoPE + attention: one node, RoPE fused into the GEMM / dq-dk epilogues
         ctx = ops.qkv_attention(h, a.in_proj.qkv_fused.weight, self._rot.table(x.device, S), a.nheads, a.kvheads,
-                                a.head_dim, doc=doc, qk_norm=a.qk_norm_args())
+                                a.head_dim, doc=doc, qk_norm=a.qk_norm_args(), qkv_bias=a.qkv_bias_arg())
         x = a.dense(ctx, residual=x)
         h, x = self.ff_ln.fork(x)
         if cfg.moe_num_experts > 0:

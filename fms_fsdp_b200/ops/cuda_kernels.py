@@ -102,7 +102,7 @@ def _try_fused_gather(a, b, layout, out, epi, residual) -> bool:
     ok = (M >= 256 and out.dtype == torch.bfloat16 and _C.get_gemm_2cta()
           and ((layout in ("nt", "nn") and epi in (0, 1)) or (layout == "tn" and epi in (0, 2, 4))
                or (layout == "nt" and epi == 5 and not req["dependent"]) or (layout == "nn" and epi == 6)
-               or (layout == "nt" and epi == 3)))
+               or (layout == "nt" and epi in (3, 8))))
     if ok and req["dependent"]:
         lo = req["full"].data_ptr() + req["begin"]
         ok = lo <= b.data_ptr() < req["full"].data_ptr() + req["end"]
@@ -178,20 +178,27 @@ def _gemm_push(a, b, tgt: PushTarget):
 
 
 # ------------------------------------------------------------------------------------------ GEMM
-def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype=None, rope=None):
+def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype=None, rope=None, bias=None):
     """``rope=(table [S, hd/2, 2] fp32, S, hd, H, KVH)``: rotary embedding of the q and k heads (the first
-    ``(H + KVH) * hd`` output columns) fused into the GEMM epilogue (QKV projection; nt layout)."""
+    ``(H + KVH) * hd`` output columns) fused into the GEMM epilogue (QKV projection; nt layout).  ``bias`` [N] (with
+    ``rope`` only): the q / k / v projection bias, added to the fp32 product before the rotation."""
     if isinstance(out, PushTarget):
         if layout != "tn" or accumulate or residual is not None:
             raise RuntimeError("the push epilogue is a plain tn (wgrad) store")
         return _gemm_push(a, b, out)
+    if bias is not None and (rope is None or layout != "nt" or accumulate or residual is not None):
+        raise ValueError("gemm: a bias is fused only with the RoPE epilogue of a plain nt projection")
     if rope is not None:
         M0 = a.shape[0]
         ok = (GEMM_IMPL == "wgmma" and layout == "nt" and a.dtype == b.dtype == torch.bfloat16 and residual is None
               and not accumulate and M0 >= 256 and M0 % 8 == 0 and _C.get_gemm_2cta() and rope[2] % 8 == 0
               and a.shape[1] % 8 == 0 and b.shape[0] % 8 == 0 and out_dtype in (None, torch.bfloat16)
-              and (out is None or out.dtype == torch.bfloat16))
-        if not ok:   # unfused: GEMM, then the in-place RoPE kernel
+              and (out is None or out.dtype == torch.bfloat16)
+              and (bias is None or (bias.dtype == torch.bfloat16 and bias.is_contiguous()
+                                    and bias.numel() == b.shape[0] and bias.data_ptr() % 4 == 0)))
+        if not ok:   # unfused: GEMM (the bias rides in the residual epilogue, row stride 0), then the in-place RoPE kernel
+            if bias is not None:
+                residual = bias.reshape(1, -1).expand(M0, b.shape[0])
             y = gemm(a, b, layout, out=out, accumulate=accumulate, residual=residual, out_dtype=out_dtype)
             table, S, hd, H, KVH = rope
             return rope_(y, table, S, H, KVH, hd)
@@ -220,8 +227,8 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
     elif accumulate:
         epi = 2
     if rope is not None:
-        epi = 3
-        _C.set_gemm_rope(rope[0], int(rope[1]), int(rope[2]), int((rope[3] + rope[4]) * rope[2]))   # for the launch below
+        epi = 3 if bias is None else 8
+        _C.set_gemm_rope(rope[0], int(rope[1]), int(rope[2]), int((rope[3] + rope[4]) * rope[2]), bias)   # for the launch below
     if _AG_QUEUE and _try_fused_gather(a, b, layout, out, epi, residual):
         return out
     _C.gemm(a, b, out, _LAYOUT[layout], epi, residual)
@@ -446,6 +453,16 @@ def qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim):
         return _fallback("qk_norm_bwd").qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim)
     dw_q, dw_k = _C.qk_norm_bwd(dqkv, xqk, rstd.contiguous(), _bf16c(w_q), _bf16c(w_k), nheads, kvheads, head_dim)
     return dw_q, dw_k
+
+
+# ------------------------------------------------------------------------------------ projection bias
+def bias_grad(dy):
+    """fp32 db[n] = sum_t dy[t, n] of a projection's output gradient [T, N], reduced in a fixed order (two runs give the
+    same bits)."""
+    if not (dy.dtype == torch.bfloat16 and dy.dim() == 2 and dy.shape[1] % 8 == 0 and dy.stride(-1) == 1
+            and dy.stride(0) % 8 == 0 and dy.data_ptr() % 16 == 0):
+        return _fallback("bias_grad").bias_grad(dy)
+    return _C.bias_grad(dy)
 
 
 # ------------------------------------------------------------------------------------- attention

@@ -307,16 +307,18 @@ class _Attention(torch.autograd.Function):
 class _QKVAttention(torch.autograd.Function):
     """QKV projection + RoPE + causal attention as ONE autograd node: the rotary embedding is the epilogue of the
     projection GEMM in forward and of the dq / dk kernels in backward, so no standalone RoPE pass touches HBM
-    (SURVEY.md K1-K3; reference path: fms MultiHeadAttention.in_proj -> RotaryEmbedding.adjusted_qk -> SDPA)."""
+    (SURVEY.md K1-K3; reference path: fms MultiHeadAttention.in_proj -> RotaryEmbedding.adjusted_qk -> SDPA).
+    ``b`` (optional, Qwen2): the [(H + 2 KVH) * hd] projection bias, added in the same epilogue before the rotation;
+    its gradient is the column sum of the un-rotated dqkv the attention backward returns."""
 
     @staticmethod
-    def forward(ctx, h, w, table, S, H, KVH, hd, scale, seg):
+    def forward(ctx, h, w, table, S, H, KVH, hd, scale, seg, b):
         K = kernels_for(h)
         B = h.shape[0]
         h2 = h.reshape(-1, h.shape[-1])
-        qkv = K.gemm(h2, _wdata(w), "nt", rope=(table, S, hd, H, KVH))
+        qkv = K.gemm(h2, _wdata(w), "nt", rope=(table, S, hd, H, KVH), bias=None if b is None else _wdata(b))
         o, lse = K.attn_fwd(qkv, B, S, H, KVH, hd, scale, seg=seg)
-        ctx.K, ctx.w, ctx.args, ctx.seg = K, w, (B, S, H, KVH, hd, scale), seg
+        ctx.K, ctx.w, ctx.b, ctx.args, ctx.seg = K, w, b, (B, S, H, KVH, hd, scale), seg
         ctx.save_for_backward(h, qkv, o, lse, table)
         return o.view(B, S, H * hd)
 
@@ -324,15 +326,18 @@ class _QKVAttention(torch.autograd.Function):
     def backward(ctx, do):
         h, qkv, o, lse, table = ctx.saved_tensors
         B, S, H, KVH, hd, scale = ctx.args
-        K, w = ctx.K, ctx.w
+        K, w, b = ctx.K, ctx.w, ctx.b
         dqkv = K.attn_bwd(do.reshape(B * S, H * hd).contiguous(), qkv, o, lse, B, S, H, KVH, hd, scale,
                           rope_table=table, seg=ctx.seg)
+        db = None
+        if b is not None and ctx.needs_input_grad[9]:
+            db = _deliver_wgrad(b, _put_fp32(K.bias_grad(dqkv)))
         h2 = h.reshape(-1, h.shape[-1])
         dh = K.gemm(dqkv, _wdata(w), "nn").view_as(h) if ctx.needs_input_grad[0] else None
         dw = None
         if ctx.needs_input_grad[1]:
             dw = _deliver_wgrad(w, lambda out, acc: K.gemm(dqkv, h2, "tn", out=out, accumulate=acc))
-        return dh, dw, None, None, None, None, None, None, None
+        return dh, dw, None, None, None, None, None, None, None, db
 
 
 def _put_fp32(val):
@@ -408,12 +413,19 @@ class _QKNormRope(torch.autograd.Function):
         return d, dwq, dwk, None, None, None, None, None, None
 
 
-def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None, qk_norm=None):
+def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None, qk_norm=None, qkv_bias=None):
     """attention(rope(h @ w^T)) for a fused [(H + 2 KVH) * hd, D] projection weight; h: [B, S, D].  ``doc``: the
     ``document_segments`` table of a packed batch (attention stays inside each document), None = causal.
-    ``qk_norm=(w_q, w_k, eps)``: per-head RMSNorm of q and k (weights [hd]) between the projection and RoPE (Qwen3)."""
+    ``qk_norm=(w_q, w_k, eps)``: per-head RMSNorm of q and k (weights [hd]) between the projection and RoPE (Qwen3).
+    ``qkv_bias``: a [(H + 2 KVH) * hd] bias of the projection, added before RoPE (Qwen2); q / k sections in the
+    interleaved pair order of the weight's rows."""
     S = h.shape[1]
     scale = (head_dim ** -0.5) if scale is None else scale
+    if qkv_bias is not None:
+        if qk_norm is not None:
+            raise ValueError("qkv_attention: qk_norm together with qkv_bias is not supported")
+        if _GEMM_PRECISION == "fp8":
+            raise NotImplementedError("qkv_attention: q / k / v projection biases are not supported with fp8 precision")
     if qk_norm is not None:
         w_q, w_k, eps = qk_norm
         if _GEMM_PRECISION == "fp8":     # fp8 projection, then the stand-alone QK-norm + RoPE kernel and attention
@@ -423,7 +435,7 @@ def qkv_attention(h, w, table, nheads, kvheads, head_dim, scale=None, doc=None, 
     if _GEMM_PRECISION == "fp8":     # fp8 projection, then the stand-alone RoPE kernel and attention
         return attention(rope_(linear(h, w), table, S, nheads, kvheads, head_dim), nheads, kvheads, head_dim, scale,
                          doc=doc)
-    return _QKVAttention.apply(h, w, table, S, nheads, kvheads, head_dim, scale, doc)
+    return _QKVAttention.apply(h, w, table, S, nheads, kvheads, head_dim, scale, doc, qkv_bias)
 
 
 def attention(qkv, nheads, kvheads, head_dim, scale=None, doc=None):

@@ -20,9 +20,10 @@ NAME = "torch"
 # GEMM family.  layout: "nt": C[M,N] = A[M,K] B[N,K]^T ; "nn": C[M,N] = A[M,K] B[K,N] ;
 #                        "tn": C[M,N] = A[K,M]^T B[K,N].  fp32 accumulate, output dtype of `out`/a.
 # ----------------------------------------------------------------------------------------------
-def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype=None, rope=None):
+def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype=None, rope=None, bias=None):
+    """``bias`` [N]: added to the product (before the rotation when ``rope`` is given: q / k / v projection biases)."""
     if rope is not None:   # (table, S, head_dim, H, KVH): RoPE on the q and k heads of a fused QKV product
-        y = gemm(a, b, layout, out=out, accumulate=accumulate, residual=residual, out_dtype=out_dtype)
+        y = gemm(a, b, layout, out=out, accumulate=accumulate, residual=residual, out_dtype=out_dtype, bias=bias)
         table, S, hd, H, KVH = rope
         return rope_(y, table, S, H, KVH, hd)
     if layout == "nt":
@@ -33,6 +34,8 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
         c = a.t() @ b
     else:
         raise ValueError(layout)
+    if bias is not None:
+        c = c + bias.to(c.dtype)
     if residual is not None:
         c = c + residual
     if out is None:
@@ -197,6 +200,14 @@ def qk_norm_bwd(dqkv, xqk, rstd, w_q, w_k, nheads, kvheads, head_dim):
     dw_q, dw_k = gx[:, :nheads].sum((0, 1)), gx[:, nheads:].sum((0, 1))
     gv.copy_(dx.to(dqkv.dtype))
     return dw_q, dw_k
+
+
+# ----------------------------------------------------------------------------------------------
+# Projection bias gradient: db[n] = sum_t dy[t, n] in fp32 (fp64 stays fp64).  For the q / k / v bias, dy is the gradient
+# of the pre-RoPE projection (the attention backward already applied the inverse rotation).
+# ----------------------------------------------------------------------------------------------
+def bias_grad(dy):
+    return _f32(dy).sum(0)
 
 
 # ----------------------------------------------------------------------------------------------

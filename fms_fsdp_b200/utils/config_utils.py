@@ -50,6 +50,14 @@ def _qwen3(emb_dim, ffn, nlayers, nheads):
                 norm_eps=1e-6, qk_norm=True, attn_head_dim=128)
 
 
+def _qwen2(emb_dim, ffn, nlayers, nheads, kvheads, vocab=151936):
+    """Qwen2 / Qwen2.5: the Llama block with q / k / v projection biases.  multiple_of=1 and grow = ffn / emb_dim give
+    hidden_dim == ffn exactly, as ``models/hf_loader.config_from_hf`` builds it."""
+    return dict(src_vocab_size=vocab, emb_dim=emb_dim, nheads=nheads, kvheads=kvheads, nlayers=nlayers,
+                hidden_grow_factor=ffn / emb_dim, multiple_of=1, max_expected_seq_len=32768, rope_theta=1000000.0,
+                norm_eps=1e-6, qkv_bias=True)
+
+
 _LLAMA_ZOO: Dict[str, Dict[str, Any]] = {
     "llama2_70b": dict(emb_dim=8192, multiple_of=4096, nheads=64, kvheads=8, nlayers=80,
                        hidden_grow_factor=28672 / 8192),
@@ -76,6 +84,12 @@ _LLAMA_ZOO: Dict[str, Dict[str, Any]] = {
     "qwen3_1.7b": _qwen3(2048, 6144, 28, 16),
     "qwen3_4b": _qwen3(2560, 9728, 36, 32),
     "qwen3_8b": _qwen3(4096, 12288, 36, 32),
+    # --- extensions: Qwen2.5 checkpoints (q / k / v biases; hf_to_fms_llama.py imports them, tied heads untied)
+    "qwen2.5_0.5b": _qwen2(896, 4864, 24, 14, 2),
+    "qwen2.5_1.5b": _qwen2(1536, 8960, 28, 12, 2),
+    "qwen2.5_3b": _qwen2(2048, 11008, 36, 16, 2),
+    "qwen2.5_7b": _qwen2(3584, 18944, 28, 28, 4, vocab=152064),
+    "qwen2_tiny": dict(_qwen2(256, 768, 2, 4, 2, vocab=1024), max_expected_seq_len=512),
     # --- extensions: sparse mixture-of-experts checkpoints (every block's feed-forward is the MoE)
     "qwen3_moe_30b_a3b": dict(_qwen3(2048, 6144, 48, 32), kvheads=4, moe_num_experts=128, moe_top_k=8,
                               moe_hidden_dim=768, moe_norm_topk=True, moe_aux_loss_coef=0.001),

@@ -6,6 +6,8 @@ recomputed?" answered before a job is queued.
 
 The numbers follow what the runtime allocates (``parallel/engine.py``) and what the autograd nodes of ``ops/functional.py`` save:
 
+* parameters of a block: the attention and feed-forward weights, the two norm gains, and with QK-norm / q / k / v biases
+  the two [hd] gains / the [(H + 2 KV) hd] bias (the bias adds no saved activation: its gradient is a column sum of dqkv);
 * state, per parameter and divided by the shard-group size: fp32 master + bf16 shard + two fp32 AdamW moments (14 B) and the
   fp32 gradient shard (4 B); unsharded (1 GPU / ddp) the gradient stays in the bf16 reduce dtype (2 B), or fp32 (4 B) when
   ``grad_accum_steps > 1`` accumulates micro-steps in it;
@@ -88,7 +90,8 @@ def plan_llama(model_variant: str, gpus: int = 1, sharding_strategy: str = "fsdp
     qk_norm = bool(getattr(c, "qk_norm", False))
     E, k, Fm = c.moe_num_experts, c.moe_top_k, c.moe_hidden_dim
     ffn_params = E * D + 3 * E * D * Fm if E > 0 else 3 * F * D
-    block_params = (qd + 2 * kvd) * D + D * qd + ffn_params + 2 * D + (2 * hd if qk_norm else 0)
+    qkv_bias = qd + 2 * kvd if getattr(c, "qkv_bias", False) else 0
+    block_params = (qd + 2 * kvd) * D + D * qd + ffn_params + 2 * D + (2 * hd if qk_norm else 0) + qkv_bias
     root_params = 2 * V * D + D
     n_params = L * block_params + root_params
 

@@ -1,5 +1,5 @@
 """Export a sharded training checkpoint to a HuggingFace ``LlamaForCausalLM`` directory (``Qwen3ForCausalLM`` for variants
-with QK-norm)
+with QK-norm, ``Qwen2ForCausalLM`` for variants with q / k / v biases)
 (CLI parity with reference ``fms_to_hf_llama.py:133-171``):
 
     python fms_to_hf_llama.py --model_variant llama2_7b --nocompiled --load_path <step_N_ckp> \
@@ -30,10 +30,15 @@ def _interleaved_to_halfsplit_vec(w: torch.Tensor) -> torch.Tensor:
     return _interleaved_to_halfsplit(w.view(-1, 1), 1).view(-1)
 
 
+def _interleaved_to_halfsplit_bias(b: torch.Tensor, nheads: int) -> torch.Tensor:
+    """A q or k projection bias [nheads * hd] in HF's half-split order, head by head like the rows."""
+    return _interleaved_to_halfsplit(b.view(-1, 1), nheads).view(-1)
+
+
 def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
     """``is_old_fms`` is kept for the reference's signature; this repo's LLaMA is always fused, pre-fusion checkpoints are
-    fused when they are read (``load_dcp_into``).  A model with ``qk_norm`` is written as a ``Qwen3ForCausalLM`` (untied
-    head), every other one as a ``LlamaForCausalLM``."""
+    fused when they are read (``load_dcp_into``).  A model with ``qk_norm`` is written as a ``Qwen3ForCausalLM``, one with
+    ``qkv_bias`` as a ``Qwen2ForCausalLM`` (both with an untied head), every other one as a ``LlamaForCausalLM``."""
     from transformers import LlamaConfig, LlamaForCausalLM
 
     c = model.config
@@ -58,6 +63,11 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
         kw.pop("mlp_bias")
         kw["head_dim"] = c.head_dim
         hf = Qwen3ForCausalLM(Qwen3Config(**kw, use_sliding_window=False))
+    elif getattr(c, "qkv_bias", False):          # Qwen2 attention: q / k / v biases, bias-free output projection
+        from transformers import Qwen2Config, Qwen2ForCausalLM
+        kw.pop("mlp_bias")
+        kw.pop("attention_bias")
+        hf = Qwen2ForCausalLM(Qwen2Config(**kw, use_sliding_window=False))
     else:
         hf = LlamaForCausalLM(LlamaConfig(**kw))
     sd = model.state_dict()
@@ -72,6 +82,12 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
             layer.self_attn.k_proj.weight.copy_(_interleaved_to_halfsplit(k, c.kv_heads))
             layer.self_attn.v_proj.weight.copy_(v)
             layer.self_attn.o_proj.weight.copy_(sd[p + "attn.dense.weight"])
+            if getattr(c, "qkv_bias", False):
+                qb, kb, vb = torch.split(sd[p + "attn.in_proj.qkv_fused.bias"],
+                                         [c.nheads * hd, c.kv_heads * hd, c.kv_heads * hd])
+                layer.self_attn.q_proj.bias.copy_(_interleaved_to_halfsplit_bias(qb, c.nheads))
+                layer.self_attn.k_proj.bias.copy_(_interleaved_to_halfsplit_bias(kb, c.kv_heads))
+                layer.self_attn.v_proj.bias.copy_(vb)
             if getattr(c, "qk_norm", False):
                 layer.self_attn.q_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.q_norm.weight"]))
                 layer.self_attn.k_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.k_norm.weight"]))

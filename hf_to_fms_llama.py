@@ -1,5 +1,5 @@
-"""Import a HuggingFace ``LlamaForCausalLM`` or ``Qwen3ForCausalLM`` directory as a single-file model checkpoint for this
-trainer -- the inverse of ``fms_to_hf_llama.py`` (the reference has only the export direction; continued pre-training /
+"""Import a HuggingFace ``LlamaForCausalLM``, ``Qwen2ForCausalLM`` or ``Qwen3ForCausalLM`` directory as a single-file model
+checkpoint for this trainer -- the inverse of ``fms_to_hf_llama.py`` (the reference has only the export direction; continued pre-training /
 fine-tuning from public weights needs the way back):
 
     python hf_to_fms_llama.py --hf_path <hf dir> --save_path llama.pth [--model_variant llama2_7b]
@@ -9,7 +9,9 @@ The file holds ``{"model_state": {<fms parameter name>: tensor}}`` -- the single
 (weights only; step count, optimizer and data-loader state start fresh, as in reference ``checkpointing_utils.py:216-233``).
 q/k rows are permuted from HF's half-split RoPE layout to the FMS interleaved-pair layout and q/k/v, gate/up are fused
 (``models/hf_loader.convert_hf_state_dict``).  Qwen3 checkpoints also carry per-head ``q_norm`` / ``k_norm`` gains, permuted
-like the q / k rows; train them with a ``qwen3_*`` variant (it has ``qk_norm`` and head_dim 128).  ``--model_variant`` is
+like the q / k rows; train them with a ``qwen3_*`` variant (it has ``qk_norm`` and head_dim 128).  Qwen2 / Qwen2.5
+checkpoints carry q / k / v biases, fused like the weights; train them with a ``qwen2.5_*`` variant (``qkv_bias``).
+``--model_variant`` is
 optional: when given, the HF config is checked against that entry of the model zoo so that a mismatch is reported here and
 not as a shape error on 8 GPUs.
 """
@@ -23,7 +25,7 @@ from fms_fsdp_b200.utils.cli import run
 from fms_fsdp_b200.utils.config_utils import get_model_config
 
 _CHECKED = ("src_vocab_size", "emb_dim", "nheads", "kv_heads", "nlayers", "hidden_dim", "rope_theta", "rope_scaling",
-            "qk_norm", "head_dim")
+            "qk_norm", "head_dim", "qkv_bias")
 
 
 def main(hf_path: str, save_path: str, model_variant: str = "", dtype: str = "bf16"):

@@ -60,6 +60,9 @@ def main(**kwargs):
     if cfg.qk_norm:
         # per-head RMSNorm of q and k before RoPE (the qwen3_* variants have it already)
         llama_config.qk_norm = True
+    if llama_config.qkv_bias and cfg.precision == "fp8":
+        raise ValueError("--precision fp8 is not supported with q / k / v projection biases (qwen2* variants): the "
+                         "fp8 projection has no bias epilogue")
     if llama_config.moe_num_experts > 0:
         if cfg.precision == "fp8":
             raise ValueError("--precision fp8 is not supported with a mixture-of-experts variant: the grouped expert "
