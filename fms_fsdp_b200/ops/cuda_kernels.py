@@ -614,8 +614,10 @@ def causal_conv1d_bwd(dy, x, w, b, seq_len, activation=True):
 
 
 # ------------------------------------------------------------------------------ Mamba2 SSD scan
-def _ssd_native_ok(x, dt, Bm, Cm, seq_len):
-    return (x.is_cuda and x.dtype == dt.dtype == Bm.dtype == Cm.dtype == torch.bfloat16 and x.dim() == 3
+def _ssd_native_ok(x, dt, Bm, Cm, seq_len, dt_softplus):
+    # Without the softplus a step's dt can be exactly 0.  The backward recovers the intra-chunk dt gradient as a column
+    # sum divided by dt (csrc/ssd.cu ssd_mask_bwd_kernel), which loses that step's term, so those inputs run on ATen.
+    return (dt_softplus and x.is_cuda and x.dtype == dt.dtype == Bm.dtype == Cm.dtype == torch.bfloat16 and x.dim() == 3
             and seq_len % 128 == 0 and x.shape[2] % 32 == 0 and Bm.shape[2] % 8 == 0 and x.shape[1] % Bm.shape[1] == 0)
 
 
@@ -625,15 +627,32 @@ def _f32c(t):
 
 def ssd_scan_fwd(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus=True):
     """Mamba2 SSD scan (csrc/ssd.cu + batched wgmma GEMMs); 128-token internal chunks whatever ``chunk_size``."""
-    if not _ssd_native_ok(x, dt, Bm, Cm, seq_len):
+    if not _ssd_native_ok(x, dt, Bm, Cm, seq_len, dt_softplus):
         return _fallback("ssd_scan_chunked").ssd_scan_chunked(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus)
     return _C.ssd_scan_fwd(x.contiguous(), dt.contiguous(), _f32c(A), Bm.contiguous(), Cm.contiguous(), _f32c(D),
                            _f32c(dt_bias), int(seq_len), bool(dt_softplus))
 
 
+def _ssd_chunked_grads(dy, x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus):
+    """(dx, ddt, dA, dB, dC, dD, ddt_bias) by autograd of the fp32 ATen chunked form."""
+    with torch.enable_grad():
+        opt = [t for t in (D, dt_bias) if t is not None]
+        leaves = [t.detach().float().requires_grad_() for t in [x, dt, A, Bm, Cm] + opt]
+        rest = iter(leaves[5:])
+        Dl = next(rest) if D is not None else None
+        bl = next(rest) if dt_bias is not None else None
+        y = torch_kernels.ssd_scan_chunked(*leaves[:5], Dl, bl, seq_len, chunk_size, dt_softplus)
+        gs = iter(torch.autograd.grad(y, leaves, dy.float()))
+    dx, ddt, dA, dB, dC = (next(gs) for _ in range(5))
+    dD = next(gs) if D is not None else None
+    dbias = next(gs) if dt_bias is not None else None
+    return dx.to(x.dtype), ddt.to(dt.dtype), dA, dB.to(Bm.dtype), dC.to(Cm.dtype), dD, dbias
+
+
 def ssd_scan_bwd(dy, x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus=True):
-    if not _ssd_native_ok(x, dt, Bm, Cm, seq_len):
-        return None                                   # caller differentiates the ATen chunked form instead
+    if not _ssd_native_ok(x, dt, Bm, Cm, seq_len, dt_softplus):
+        _fallback("ssd_scan_bwd")
+        return _ssd_chunked_grads(dy, x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus)
     dx, ddt, dA, dB, dC, dD, dbias = _C.ssd_scan_bwd(dy.contiguous(), x.contiguous(), dt.contiguous(), _f32c(A),
                                                      Bm.contiguous(), Cm.contiguous(), _f32c(D), _f32c(dt_bias),
                                                      int(seq_len), bool(dt_softplus))

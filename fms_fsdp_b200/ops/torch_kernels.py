@@ -626,29 +626,34 @@ def causal_conv1d_bwd(dy, x, w, b, seq_len, activation=True):
     return dx.transpose(1, 2).reshape(M, C).to(x.dtype), dw, db
 
 
+def _hi(t):
+    """fp32 compute for the Mamba oracles, float64 kept as float64 (the CPU tests differentiate them in float64)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 def ssd_scan_fwd(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softplus=True):
     """Mamba2 state-space-dual scan (sequential fp32 oracle; the CUDA kernel is chunked).
     x: [M, H, P]; dt: [M, H]; A: [H] (negative); Bm, Cm: [M, G, N]; D: [H]; returns y [M, H, P]."""
     M, H, P = x.shape
     Bsz = M // seq_len
     G, N = Bm.shape[1], Bm.shape[2]
-    xf = x.float().view(Bsz, seq_len, H, P)
-    dtf = dt.float().view(Bsz, seq_len, H)
+    xf = _hi(x).view(Bsz, seq_len, H, P)
+    dtf = _hi(dt).view(Bsz, seq_len, H)
     if dt_bias is not None:
-        dtf = dtf + dt_bias.float()
+        dtf = dtf + _hi(dt_bias)
     if dt_softplus:
         dtf = F.softplus(dtf)
-    Bf = Bm.float().view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
-    Cf = Cm.float().view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
-    dA = torch.exp(dtf * A.float())  # [B,S,H]
-    state = torch.zeros(Bsz, H, P, N, dtype=torch.float32, device=x.device)
+    Bf = _hi(Bm).view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
+    Cf = _hi(Cm).view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
+    dA = torch.exp(dtf * _hi(A))  # [B,S,H]
+    state = torch.zeros(Bsz, H, P, N, dtype=xf.dtype, device=x.device)
     ys = []
     for t in range(seq_len):
         state = state * dA[:, t, :, None, None] + (dtf[:, t, :, None] * xf[:, t])[..., None] * Bf[:, t, :, None, :]
         ys.append((state * Cf[:, t, :, None, :]).sum(-1))
     y = torch.stack(ys, dim=1)
     if D is not None:
-        y = y + xf * D.float()[None, None, :, None]
+        y = y + xf * _hi(D)[None, None, :, None]
     return y.reshape(M, H, P).to(x.dtype)
 
 
@@ -669,21 +674,21 @@ def ssd_scan_chunked(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softp
     G, N = Bm.shape[1], Bm.shape[2]
     L = min(chunk_size, seq_len)
     pad = (-seq_len) % L
-    xf = x.float().view(Bsz, seq_len, H, P)
-    dtf = dt.float().view(Bsz, seq_len, H)
+    xf = _hi(x).view(Bsz, seq_len, H, P)
+    dtf = _hi(dt).view(Bsz, seq_len, H)
     if dt_bias is not None:
-        dtf = dtf + dt_bias.float()
+        dtf = dtf + _hi(dt_bias)
     if dt_softplus:
         dtf = F.softplus(dtf)
-    Bf = Bm.float().view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
-    Cf = Cm.float().view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
+    Bf = _hi(Bm).view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
+    Cf = _hi(Cm).view(Bsz, seq_len, G, N).repeat_interleave(H // G, dim=2)
     if pad:
         xf, dtf = F.pad(xf, (0, 0, 0, 0, 0, pad)), F.pad(dtf, (0, 0, 0, pad))
         Bf, Cf = F.pad(Bf, (0, 0, 0, 0, 0, pad)), F.pad(Cf, (0, 0, 0, 0, 0, pad))
     S2 = seq_len + pad
     nc = S2 // L
     X = (xf * dtf.unsqueeze(-1)).view(Bsz, nc, L, H, P)
-    Ad = (dtf * A.float()).view(Bsz, nc, L, H).permute(0, 3, 1, 2)        # [b,h,c,L]
+    Ad = (dtf * _hi(A)).view(Bsz, nc, L, H).permute(0, 3, 1, 2)        # [b,h,c,L]
     Bc = Bf.view(Bsz, nc, L, H, N)
     Cc = Cf.view(Bsz, nc, L, H, N)
     A_cs = torch.cumsum(Ad, dim=-1)
@@ -697,7 +702,7 @@ def ssd_scan_chunked(x, dt, A, Bm, Cm, D, dt_bias, seq_len, chunk_size, dt_softp
     Y_off = torch.einsum("bclhn,bchpn,bhcl->bclhp", Cc, new_states, torch.exp(A_cs))
     y = (Y_diag + Y_off).reshape(Bsz, S2, H, P)[:, :seq_len]
     if D is not None:
-        y = y + xf[:, :seq_len] * D.float()[None, None, :, None]
+        y = y + xf[:, :seq_len] * _hi(D)[None, None, :, None]
     return y.reshape(M, H, P).to(x.dtype)
 
 
@@ -706,22 +711,22 @@ def selective_scan_fwd(u, delta, A, Bm, Cm, D, z, delta_bias, seq_len, delta_sof
     M, Dm = u.shape
     Bsz = M // seq_len
     N = A.shape[1]
-    uf = u.float().view(Bsz, seq_len, Dm)
-    df = delta.float().view(Bsz, seq_len, Dm)
+    uf = _hi(u).view(Bsz, seq_len, Dm)
+    df = _hi(delta).view(Bsz, seq_len, Dm)
     if delta_bias is not None:
-        df = df + delta_bias.float()
+        df = df + _hi(delta_bias)
     if delta_softplus:
         df = F.softplus(df)
-    Bf = Bm.float().view(Bsz, seq_len, N)
-    Cf = Cm.float().view(Bsz, seq_len, N)
-    h = torch.zeros(Bsz, Dm, N, dtype=torch.float32, device=u.device)
+    Bf = _hi(Bm).view(Bsz, seq_len, N)
+    Cf = _hi(Cm).view(Bsz, seq_len, N)
+    h = torch.zeros(Bsz, Dm, N, dtype=uf.dtype, device=u.device)
     ys = []
     for t in range(seq_len):
-        h = h * torch.exp(df[:, t, :, None] * A.float()) + (df[:, t] * uf[:, t])[..., None] * Bf[:, t, None, :]
+        h = h * torch.exp(df[:, t, :, None] * _hi(A)) + (df[:, t] * uf[:, t])[..., None] * Bf[:, t, None, :]
         ys.append((h * Cf[:, t, None, :]).sum(-1))
     y = torch.stack(ys, dim=1)
     if D is not None:
-        y = y + uf * D.float()
+        y = y + uf * _hi(D)
     if z is not None:
-        y = y * F.silu(z.float().view(Bsz, seq_len, Dm))
+        y = y * F.silu(_hi(z).view(Bsz, seq_len, Dm))
     return y.reshape(M, Dm).to(u.dtype)

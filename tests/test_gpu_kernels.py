@@ -222,9 +222,10 @@ def test_ssd_scan_native_vs_chunked_oracle(K, shape):
     y0 = TK.ssd_scan_chunked(x, dt, A, Bm, Cm, D, bias, S, 128)
     g0 = torch.autograd.grad(y0, [x, dt, A, Bm, Cm, D, bias], dy.float())
     d = lambda t: t.detach()
+    f0 = CK.fallback_count()
     y1 = CK.ssd_scan_fwd(d(x), d(dt), d(A), d(Bm), d(Cm), d(D), d(bias), S, 256)
     g1 = CK.ssd_scan_bwd(dy, d(x), d(dt), d(A), d(Bm), d(Cm), d(D), d(bias), S, 256)
-    assert g1 is not None, "native SSD path was not taken"
+    assert CK.fallback_count() == f0, "native SSD path was not taken"
     assert rel(y1, y0) < 2e-2
     for name, a, b in zip(["dx", "ddt", "dA", "dB", "dC", "dD", "dbias"], g1, g0):
         assert rel(a, b) < 3e-2, name
