@@ -6,15 +6,16 @@
 
 #include <cmath>
 #include <cstdint>
+#include <string>
+
+#include "gemm_epilogue.h"
 
 #define DECL extern "C"
-DECL int b200_gemm_bf16(const void*, const void*, void*, const void*, int, int, int, int, int, int, int, int, int, int,
-                        int, cudaStream_t);
 DECL int b200_gemm2_bf16(const void*, const void*, void*, const void*, int, int, int, int, int, int, int, int, int, int,
-                         int, cudaStream_t);
+                         int, const GemmEpilogueArgs&, cudaStream_t);
 DECL int b200_gemm2_ag_bf16(const void*, const void*, void*, const void*, int, int, int, int, int, int, int, int, int, int,
-                            const void* const*, void*, unsigned long long, unsigned long long, unsigned long long, int, int,
-                            uint32_t*, uint32_t, int, cudaStream_t);
+                            const GemmEpilogueArgs&, const void* const*, void*, unsigned long long, unsigned long long,
+                            unsigned long long, int, int, uint32_t*, uint32_t, int, cudaStream_t);
 DECL int b200_bgemm_bf16(const void*, const void*, void*, int, int, int, int, int, int, int, int, long long, long long,
                          long long, long long, long long, long long, int, int, int, int, cudaStream_t);
 DECL int b200_ssd_prep(const void*, const float*, const float*, float*, float*, float*, int, int, int, cudaStream_t);
@@ -71,12 +72,9 @@ DECL int b200_attn_bwd_lockstep(const void*, const void*, const void*, const flo
                                 int, float, const float*, cudaStream_t, const int*);
 DECL int b200_bias_grad_slices(int, int);
 DECL int b200_bias_grad(const void*, float*, float*, int, int, int, cudaStream_t);
-DECL void b200_gemm2_set_rope(const float*, int, int, int, const void*);
-DECL void b200_gemm2_set_swiglu(void*, int, int, int);
 DECL void b200_gemm2_set_tile(int);
 DECL int b200_gemm2_fp8(const void*, const void*, void*, const float*, const float*, int, int, int, int, int, int, cudaStream_t);
 DECL int b200_quant_rowwise_e4m3(const void*, void*, float*, int, int, int, int, cudaStream_t);
-DECL void b200_gemm2_set_push(void* const*, long long, long long, int, int, int);
 DECL int b200_p2p_push_range(const void*, void* const*, long long, long long, long long, int, cudaStream_t);
 DECL int b200_p2p_allgather(const void* const*, void*, long long, int, int, cudaStream_t);
 DECL int b200_reduce_scatter(const void* const*, float*, long long, long long, int, int, int, float, float*, int,
@@ -86,7 +84,7 @@ DECL int b200_signal_barrier(uint32_t* const*, int, int, uint32_t, int, int, cud
 DECL int b200_scalar_allreduce_bytes();
 DECL int b200_scalar_allreduce(uint8_t* const*, int, int, uint32_t, float*, int, cudaStream_t);
 DECL int b200_gemm_grouped_bf16(const void*, const void*, void*, const int*, const int*, int, int, int, int, int, int, int,
-                                int, int, int, int, cudaStream_t);
+                                int, int, int, int, const GemmEpilogueArgs&, cudaStream_t);
 DECL int b200_moe_route(const float*, int, int, int, int, float*, int*, float*, cudaStream_t);
 DECL int b200_moe_plan_ws_chunks(int);
 DECL int b200_moe_plan(const int*, const float*, int, int, int, int, int*, float*, int*, int*, int*, int*, int*, float*,
@@ -106,8 +104,6 @@ namespace {
 
 static int64_t g_launches = 0;
 static int g_reduce_ctas_default = 264;  // 2 CTAs per SM of an H100
-static bool g_gemm_2cta = true;
-static int64_t g_rope_bias_n = -1;        // length of the bias of the next RoPE-bias GEMM (-1: none set)
 
 inline cudaStream_t cur_stream() { return at::cuda::getCurrentCUDAStream().stream(); }
 
@@ -126,9 +122,65 @@ inline void need_rowmajor2d(const at::Tensor& t, const char* name) {
               name, " must be 16-byte aligned (ptr and row stride)");
 }
 
-// layout: 0 = nt, 1 = nn, 2 = tn ; epi: 0 store, 1 +residual, 2 accumulate into c
+// The operands of the fused epilogues, given by keyword with each GEMM launch (None = not given).  n: N of the launch.
+//   RoPE (epi 3, 8):    rope_table [S, hd/2, 2] fp32, rope_S, rope_hd, rope_cols (the first rope_cols columns rotate);
+//                       bias [N] bf16 (epi 8), added before the rotation
+//   SwiGLU (epi 5, 6):  aux = the activation output [M, F] (5) or the saved projection [M, 2F] (6), swiglu_F, gate_first
+//   push (epi 4):       push_bases (int64 CUDA table of every rank's staging-buffer base), push_n (elements per shard),
+//                       push_off, push_rank, push_bulk, push_world (> 1 rotates the tile raster by rank / world of a sweep)
+GemmEpilogueArgs epilogue_args(const py::kwargs& kw, int64_t n) {
+  GemmEpilogueArgs e;
+  at::Tensor table, bias, aux, bases;
+  for (const auto& item : kw) {
+    const std::string key = py::str(item.first);
+    const py::handle v = item.second;
+    if (v.is_none()) continue;
+    if (key == "rope_table") table = v.cast<at::Tensor>();
+    else if (key == "rope_S") e.rope_S = v.cast<int>();
+    else if (key == "rope_hd") e.rope_hd = v.cast<int>();
+    else if (key == "rope_cols") e.rope_cols = v.cast<int>();
+    else if (key == "bias") bias = v.cast<at::Tensor>();
+    else if (key == "aux") aux = v.cast<at::Tensor>();
+    else if (key == "swiglu_F") e.swi_F = v.cast<int>();
+    else if (key == "gate_first") e.gate_first = v.cast<bool>() ? 1 : 0;
+    else if (key == "push_bases") bases = v.cast<at::Tensor>();
+    else if (key == "push_n") e.push_n = v.cast<long long>();
+    else if (key == "push_off") e.push_off = v.cast<long long>();
+    else if (key == "push_rank") e.push_rank = v.cast<int>();
+    else if (key == "push_bulk") e.push_bulk = v.cast<bool>() ? 1 : 0;
+    else if (key == "push_world") e.push_world = v.cast<int>();
+    else TORCH_CHECK(false, "unknown GEMM epilogue argument '", key, "'");
+  }
+  if (table.defined()) {
+    need(table, "rope table", at::kFloat);
+    TORCH_CHECK(table.is_contiguous() && table.numel() >= (int64_t)e.rope_S * e.rope_hd,
+                "rope table must be [S, hd/2, 2] fp32");
+    e.rope_table = table.data_ptr<float>();
+  }
+  if (bias.defined()) {
+    need(bias, "qkv bias", at::kBFloat16);
+    TORCH_CHECK(bias.dim() == 1 && bias.is_contiguous() && (reinterpret_cast<uintptr_t>(bias.data_ptr()) & 3) == 0 &&
+                bias.numel() == n, "qkv bias must be a contiguous, 4-byte aligned [N] vector, N = ", n);
+    e.bias = bias.data_ptr();
+  }
+  if (aux.defined()) {
+    need(aux, "aux", at::kBFloat16);
+    TORCH_CHECK(aux.dim() == 2 && aux.stride(1) == 1 && (aux.size(1) == e.swi_F || aux.size(1) == 2 * e.swi_F),
+                "SwiGLU aux must be 2-D with unit inner stride and F or 2F columns");
+    e.aux = aux.data_ptr();
+    e.ld_aux = (int)aux.stride(0);
+  }
+  if (bases.defined()) {
+    TORCH_CHECK(bases.is_cuda() && bases.scalar_type() == at::kLong && bases.is_contiguous(), "push table: int64 CUDA tensor");
+    e.push_bases = (void* const*)bases.data_ptr();
+  }
+  return e;
+}
+
+// layout: 0 = nt, 1 = nn, 2 = tn ; epi: 0 store, 1 +residual, 2 accumulate into c, 3 / 8 RoPE (/ with bias),
+// 5 / 6 SwiGLU forward / backward; the fused epilogues take their operands by keyword (epilogue_args)
 void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layout, int64_t epi,
-          const c10::optional<at::Tensor>& residual) {
+          const c10::optional<at::Tensor>& residual, const py::kwargs& epi_kw) {
   c10::cuda::CUDAGuard guard(a.device());
   need(a, "a", at::kBFloat16);
   need(b, "b", at::kBFloat16);
@@ -149,8 +201,8 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layou
   }
   TORCH_CHECK(c.size(0) == M && c.size(1) == (epi == 6 ? 2 * N : N), "c shape mismatch");
   TORCH_CHECK(K % 8 == 0 && N % 8 == 0 && M % 8 == 0, "M, N, K must be multiples of 8");
-  TORCH_CHECK((epi != 5 && epi != 6) || (g_gemm_2cta && M >= 256 && c.scalar_type() == at::kBFloat16),
-              "SwiGLU epilogues: M >= 256, bf16 output (call set_gemm_swiglu first)");
+  TORCH_CHECK((epi != 5 && epi != 6) || (M >= 256 && c.scalar_type() == at::kBFloat16),
+              "SwiGLU epilogues: M >= 256, bf16 output");
   const void* r = nullptr;
   int ldr = 0;
   if (epi == 1) {
@@ -160,20 +212,13 @@ void gemm(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, int64_t layou
     r = residual->data_ptr();
     ldr = residual->stride(0);
   }
-  TORCH_CHECK((epi != 3 && epi != 8) || (g_gemm_2cta && M >= 256 && layout == 0 && c.scalar_type() == at::kBFloat16),
-              "RoPE epilogue: M >= 256, nt layout, bf16 output only (call set_gemm_rope first)");
-  TORCH_CHECK(epi != 8 || g_rope_bias_n == N, "RoPE-bias epilogue: set_gemm_rope(..., bias) with a [N] bias first");
+  TORCH_CHECK((epi != 3 && epi != 8) || (M >= 256 && layout == 0 && c.scalar_type() == at::kBFloat16),
+              "RoPE epilogue: M >= 256, nt layout, bf16 output only");
   TORCH_CHECK(epi != 4, "push epilogue: use gemm_push (no output tensor)");
-  // fused-epilogue entry for anything with at least 256 rows; the store / residual / accumulate entry otherwise
-  if (g_gemm_2cta && M >= 256) {
-    check(b200_gemm2_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0),
-                          ldr, a_mn, b_mn, (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()),
-          "gemm2_bf16_wgmma");
-    return;
-  }
-  check(b200_gemm_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0),
-                       ldr, a_mn, b_mn, (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()),
-        "gemm_bf16_wgmma");
+  check(b200_gemm2_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0), ldr,
+                        a_mn, b_mn, (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, epilogue_args(epi_kw, N),
+                        cur_stream()),
+        "gemm2_bf16_wgmma");
 }
 
 std::vector<at::Tensor> rmsnorm_fwd(const at::Tensor& x, const at::Tensor& w, double eps) {
@@ -563,28 +608,27 @@ std::vector<at::Tensor> causal_conv1d_bwd(const at::Tensor& dy, const at::Tensor
   return {dx, dw, db};
 }
 
-void set_gemm_2cta(bool on) { g_gemm_2cta = on; }
-bool get_gemm_2cta() { return g_gemm_2cta; }
 // GEMM with the all-gather of a unit's parameters fused in (comm warps over NVLink peer memory)
 void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::Tensor>& c_opt, int64_t layout, int64_t epi,
              const c10::optional<at::Tensor>& residual, const at::Tensor& peer_ptrs, at::Tensor& full,
              int64_t shard_bytes, int64_t begin, int64_t end, int64_t world, int64_t rank, at::Tensor& flags,
-             int64_t epoch, bool dependent) {
+             int64_t epoch, bool dependent, const py::kwargs& epi_kw) {
   c10::cuda::CUDAGuard guard(a.device());
   need(a, "a", at::kBFloat16);
   need(b, "b", at::kBFloat16);
   need(flags, "flags", at::kInt);
   need_rowmajor2d(a, "a");
   need_rowmajor2d(b, "b");
-  if (epi == 4) {   // push epilogue: the output goes to the owners' staging slots (set_gemm_push), there is no C
+  if (epi == 4) {   // push epilogue: the output goes to the owners' staging slots (push_bases), there is no C
     TORCH_CHECK(layout == 2 && !c_opt.has_value(), "push epilogue: tn layout, no output tensor");
     const int K = a.size(0), M = a.size(1), N = b.size(1);
     TORCH_CHECK(b.size(0) == K && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0);
+    const GemmEpilogueArgs ea = epilogue_args(epi_kw, N);
     check(b200_gemm2_ag_bf16(a.data_ptr(), b.data_ptr(), nullptr, nullptr, M, N, K, a.stride(0), b.stride(0), N, 0, 1, 1, 4,
-                             (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(), (unsigned long long)shard_bytes,
+                             ea, (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(), (unsigned long long)shard_bytes,
                              (unsigned long long)begin, (unsigned long long)end, (int)world, (int)rank,
                              (uint32_t*)flags.data_ptr(), (uint32_t)epoch, dependent ? 1 : 0, cur_stream()),
-          "gemm2_ag_push_bf16_wgmma");
+          "gemm2_push_ag_bf16_wgmma");
     return;
   }
   TORCH_CHECK(c_opt.has_value(), "gemm_ag: output tensor required");
@@ -596,7 +640,7 @@ void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::T
   else if (layout == 1) { M = a.size(0); K = a.size(1); N = b.size(1); b_mn = 1; TORCH_CHECK(b.size(0) == K); }
   else { K = a.size(0); M = a.size(1); N = b.size(1); a_mn = b_mn = 1; TORCH_CHECK(b.size(0) == K); }
   TORCH_CHECK(c.size(0) == M && c.size(1) == (epi == 6 ? 2 * N : N) && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0);
-  TORCH_CHECK(epi != 8 || g_rope_bias_n == N, "RoPE-bias epilogue: set_gemm_rope(..., bias) with a [N] bias first");
+  const GemmEpilogueArgs ea = epilogue_args(epi_kw, N);
   const void* r = nullptr;
   int ldr = 0;
   if (epi == 1) {
@@ -606,23 +650,23 @@ void gemm_ag(const at::Tensor& a, const at::Tensor& b, const c10::optional<at::T
     ldr = residual->stride(0);
   }
   check(b200_gemm2_ag_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), r, M, N, K, a.stride(0), b.stride(0), c.stride(0), ldr,
-                           a_mn, b_mn, (int)epi, (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(),
+                           a_mn, b_mn, (int)epi, ea, (const void* const*)peer_ptrs.data_ptr(), full.data_ptr(),
                            (unsigned long long)shard_bytes, (unsigned long long)begin, (unsigned long long)end, (int)world,
                            (int)rank, (uint32_t*)flags.data_ptr(), (uint32_t)epoch, dependent ? 1 : 0, cur_stream()),
         "gemm2_ag_bf16_wgmma");
 }
 // wgrad GEMM (tn: dW[M,N] = a[K,M]^T b[K,N]) whose epilogue pushes every tile to the owning rank's staging slot
-void gemm_push(const at::Tensor& a, const at::Tensor& b) {
+void gemm_push(const at::Tensor& a, const at::Tensor& b, const py::kwargs& epi_kw) {
   c10::cuda::CUDAGuard guard(a.device());
   need(a, "a", at::kBFloat16);
   need(b, "b", at::kBFloat16);
   need_rowmajor2d(a, "a");
   need_rowmajor2d(b, "b");
   const int K = a.size(0), M = a.size(1), N = b.size(1);
-  TORCH_CHECK(b.size(0) == K && g_gemm_2cta && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0,
+  TORCH_CHECK(b.size(0) == K && M >= 256 && K % 8 == 0 && N % 8 == 0 && M % 8 == 0,
               "push epilogue: M >= 256, dims multiples of 8");
   check(b200_gemm2_bf16(a.data_ptr(), b.data_ptr(), nullptr, nullptr, M, N, K, a.stride(0), b.stride(0), N, 0, 1, 1, 4, 0,
-                        cur_stream()), "gemm2_push_bf16_wgmma");
+                        epilogue_args(epi_kw, N), cur_stream()), "gemm2_push_bf16_wgmma");
 }
 // optional fp8 forward path: row-wise e4m3 quantisation and the e4m3 x e4m3 -> bf16 GEMM (kind::f8f6f4)
 std::vector<at::Tensor> quant_rowwise_e4m3(const at::Tensor& x) {
@@ -1008,9 +1052,9 @@ at::Tensor moe_route_bwd(const at::Tensor& probs, const at::Tensor& ids, const a
 
 // layout 0 (nt) / 1 (nn): m-grouped, a = the permuted rows [Mpad, K], b = the expert weights [E, rows, cols]; c [Mpad, *].
 // layout 2 (tn): k-grouped wgrad, a [Mpad, M], b [Mpad, N], c [E, M, N].  epi 0 store, 2 accumulate (tn), 5 SwiGLU (nt),
-// 6 SwiGLU backward (nn); the SwiGLU epilogues read set_gemm_swiglu like the dense GEMM.
+// 6 SwiGLU backward (nn); the SwiGLU epilogues take aux / swiglu_F / gate_first by keyword like the dense GEMM.
 void gemm_grouped(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, const at::Tensor& plan, int64_t T, int64_t k,
-                  int64_t layout, int64_t epi) {
+                  int64_t layout, int64_t epi, const py::kwargs& epi_kw) {
   c10::cuda::CUDAGuard guard(a.device());
   need(a, "a", at::kBFloat16);
   need(b, "b", at::kBFloat16);
@@ -1036,7 +1080,8 @@ void gemm_grouped(const at::Tensor& a, const at::Tensor& b, at::Tensor& c, const
   const int ldc = layout == 2 ? N : (int)c.stride(0);
   check(b200_gemm_grouped_bf16(a.data_ptr(), b.data_ptr(), c.data_ptr(), q.tile, q.start, E, d.Mpad, M, N, K,
                                (int)a.stride(0), layout == 2 ? (int)b.stride(0) : (int)b.stride(1), ldc, (int)layout,
-                               (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, cur_stream()), "gemm_grouped_bf16");
+                               (int)epi, c.scalar_type() == at::kFloat ? 1 : 0, epilogue_args(epi_kw, N), cur_stream()),
+        "gemm_grouped_bf16");
 }
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
@@ -1090,22 +1135,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("causal_conv1d_fwd", &causal_conv1d_fwd);
   m.def("causal_conv1d_bwd", &causal_conv1d_bwd);
   m.def("set_reduce_ctas", [](int64_t n) { g_reduce_ctas_default = n < 1 ? 1 : (int)n; b200_comm_set_reduce_ctas((int)n); });
-  m.def("set_gemm_rope", [](const at::Tensor& table, int64_t S, int64_t hd, int64_t cols,
-                            const c10::optional<at::Tensor>& bias) {
-    // bias: the [N] bf16 q / k / v bias the next RoPE-bias GEMM (epi 8) adds before the rotation
-    need(table, "rope table", at::kFloat);
-    TORCH_CHECK(table.is_contiguous() && table.numel() >= S * hd, "rope table must be [S, hd/2, 2] fp32");
-    const void* b = nullptr;
-    g_rope_bias_n = -1;
-    if (bias.has_value() && bias->defined()) {
-      need(*bias, "qkv bias", at::kBFloat16);
-      TORCH_CHECK(bias->dim() == 1 && bias->is_contiguous() && (reinterpret_cast<uintptr_t>(bias->data_ptr()) & 3) == 0,
-                  "qkv bias must be a contiguous, 4-byte aligned [N] vector");
-      b = bias->data_ptr();
-      g_rope_bias_n = bias->numel();
-    }
-    b200_gemm2_set_rope(table.data_ptr<float>(), (int)S, (int)hd, (int)cols, b);
-  }, py::arg("table"), py::arg("S"), py::arg("hd"), py::arg("cols"), py::arg("bias") = py::none());
   m.def("push_range", [](const at::Tensor& src, const at::Tensor& bases, int64_t n, int64_t off, int64_t rank) {
     // this rank's gradient elements [off, off + src.numel()) -> the owners' staging slots (norm gains / biases)
     c10::cuda::CUDAGuard guard(src.device());
@@ -1114,24 +1143,10 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
     check(b200_p2p_push_range(src.data_ptr(), (void* const*)bases.data_ptr(), n, off, src.numel(), (int)rank, cur_stream()),
           "p2p_push_range");
   });
-  m.def("set_gemm_swiglu", [](const at::Tensor& aux, int64_t F, bool gate_first) {
-    // aux: activation output [M, F] (epi 5, forward) or the saved bf16 projection [M, 2F] (epi 6, backward)
-    need(aux, "aux", at::kBFloat16);
-    TORCH_CHECK(aux.dim() == 2 && aux.stride(1) == 1 && (aux.size(1) == F || aux.size(1) == 2 * F));
-    b200_gemm2_set_swiglu(aux.data_ptr(), (int)aux.stride(0), (int)F, gate_first ? 1 : 0);
-  });
-  m.def("set_gemm_push", [](const at::Tensor& bases, int64_t n, int64_t off, int64_t rank, bool bulk, int64_t rot_world) {
-    // int64 device table of every rank's staging-buffer base address (fused wgrad GEMM -> reduce-scatter);
-    // rot_world > 1 rotates the tile raster by rank / rot_world of a sweep (spreads the pushes over all owners)
-    TORCH_CHECK(bases.is_cuda() && bases.scalar_type() == at::kLong && bases.is_contiguous(), "push table: int64 CUDA tensor");
-    b200_gemm2_set_push((void* const*)bases.data_ptr(), n, off, (int)rank, bulk ? 1 : 0, (int)rot_world);
-  }, py::arg("bases"), py::arg("n"), py::arg("off"), py::arg("rank"), py::arg("bulk") = true, py::arg("rot_world") = 1);
   m.def("ssd_scan_fwd", &ssd_scan_fwd);
   m.def("selective_scan_fwd", &selective_scan_fwd);
   m.def("selective_scan_bwd", &selective_scan_bwd);
   m.def("ssd_scan_bwd", &ssd_scan_bwd);
-  m.def("set_gemm_2cta", &set_gemm_2cta);
-  m.def("get_gemm_2cta", &get_gemm_2cta);
   // private: pins the tile of the single-GPU GEMMs (0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256) so that the
   // GEMM benchmark and the tests can compare both tiles on the same operands
   m.def("_set_gemm_tile", [](int64_t mode) { b200_gemm2_set_tile((int)mode); });

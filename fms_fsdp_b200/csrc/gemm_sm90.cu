@@ -17,7 +17,11 @@
 //
 // gemm_wide_bf16 is the same pipeline on a 128 x 256 tile (wgmma m64n256k16) for the GEMMs without fused communication;
 // use_wide picks the tile per launch.
+//
+// The operands of the fused epilogues (RoPE table and bias, SwiGLU aux, push table) come with each launch in a
+// GemmEpilogueArgs (gemm_epilogue.h); check_epilogue validates them for all three launch entries.
 #include "common.cuh"
+#include "gemm_epilogue.h"
 #include "tensormap.h"
 #include "wgmma.cuh"
 
@@ -737,57 +741,45 @@ static int make_maps(CUtensorMap* tmA, CUtensorMap* tmB, const void* A, const vo
   return 0;
 }
 
-// RoPE epilogue parameters of the NEXT epi == EPI_ROPE / EPI_ROPE_BIAS launch (set immediately before it by the single
-// host thread that owns the stream; keeps the launcher signatures unchanged)
-static const float* g_rope_table = nullptr;
-static const __nv_bfloat16* g_rope_bias = nullptr;
-static int g_rope_S = 1, g_rope_hd = 2, g_rope_cols = 0;
-// same convention for the push epilogue
-static void* const* g_push_bases = nullptr;
-static long long g_push_n = 1, g_push_off = 0;
-static int g_push_rank = 0, g_push_bulk = 1, g_push_world = 1;
-// same convention for the SwiGLU epilogues: aux = activation output (forward) / saved projection (backward)
-static void* g_swi_aux = nullptr;
-static int g_swi_ld = 0, g_swi_F = 0, g_swi_gate_first = 1;
-
-static GemmParams make_params(void* C, const void* R, int M, int N, int K, int ldc, int ldr, int epi) {
+static GemmParams make_params(void* C, const void* R, int M, int N, int K, int ldc, int ldr, int epi,
+                              const GemmEpilogueArgs& e) {
   GemmParams p{};
   p.M = M; p.N = N; p.K = K; p.ldc = ldc; p.ldr = ldr; p.C = C; p.R = R;
   p.m_tiles = (M + BM - 1) / BM;
   p.n_tiles = (N + BN - 1) / BN;
   p.nb0 = p.nb1 = 1;
-  p.rope = g_rope_table; p.rope_S = g_rope_S; p.rope_hd = g_rope_hd; p.rope_cols = g_rope_cols;
-  p.push_bases = g_push_bases; p.push_n = g_push_n; p.push_off = g_push_off; p.push_rank = g_push_rank;
-  p.push_bulk = g_push_bulk;
-  p.aux = g_swi_aux; p.ld_aux = g_swi_ld; p.swi_F = g_swi_F; p.swi_gate_first = g_swi_gate_first;
-  if (epi == EPI_ROPE_BIAS) p.bias = g_rope_bias;
-  if (epi == EPI_PUSH && g_push_world > 1) {
+  p.rope = e.rope_table; p.rope_S = e.rope_S; p.rope_hd = e.rope_hd; p.rope_cols = e.rope_cols;
+  p.push_bases = e.push_bases; p.push_n = e.push_n; p.push_off = e.push_off; p.push_rank = e.push_rank;
+  p.push_bulk = e.push_bulk;
+  p.aux = e.aux; p.ld_aux = e.ld_aux; p.swi_F = e.swi_F; p.swi_gate_first = e.gate_first;
+  if (epi == EPI_ROPE_BIAS) p.bias = static_cast<const __nv_bfloat16*>(e.bias);
+  if (epi == EPI_PUSH && e.push_world > 1) {
     const int per_band = GROUP_M * p.n_tiles, tiles = p.m_tiles * p.n_tiles;
     const int bands = (tiles + per_band - 1) / per_band;
-    p.tile_rot = (int)(((long long)(g_push_rank % g_push_world) * bands / g_push_world) * per_band) % tiles;
+    p.tile_rot = (int)(((long long)(e.push_rank % e.push_world) * bands / e.push_world) * per_band) % tiles;
   }
   return p;
 }
 
+// The operand checks of the fused epilogues, for every launch entry.  Returns 0 or the epilogue's error code:
+// -11 SwiGLU, -12 SwiGLU backward, -8 RoPE (with or without bias), -9 push.
+static int check_epilogue(const GemmEpilogueArgs& e, int epi, int N, int ldc, int a_mn, int b_mn, int out_fp32) {
+  if (epi == EPI_SWIGLU &&   // nt; N = 2F rows of the fused weight, tiles of 64 features
+      (a_mn || b_mn || out_fp32 || !e.aux || e.swi_F <= 0 || N != 2 * e.swi_F || (e.swi_F % 64) || (e.ld_aux % 8)))
+    return -11;
+  if (epi == EPI_SWIGLU_BWD &&   // nn; N = F columns of dS, output [M, 2F]
+      (a_mn || !b_mn || out_fp32 || !e.aux || e.swi_F != N || (N % 8) || (e.ld_aux % 8)))
+    return -12;
+  if ((epi == EPI_ROPE || epi == EPI_ROPE_BIAS) && (a_mn || b_mn || out_fp32 || !e.rope_table || (e.rope_hd % 8) ||
+                                                    (e.rope_cols % 8) || (epi == EPI_ROPE_BIAS && !e.bias)))
+    return -8;
+  if (epi == EPI_PUSH &&   // wgrad (tn) only; every 8-element vector must stay inside one owner's slice
+      (!a_mn || !b_mn || out_fp32 || !e.push_bases || e.push_n <= 0 || (e.push_n % 8) || (e.push_off % 8) || (ldc % 8)))
+    return -9;
+  return 0;
+}
+
 }  // namespace b200
-
-// bias: [N] bf16, 4-byte aligned, read by EPI_ROPE_BIAS launches only (nullptr otherwise)
-extern "C" void b200_gemm2_set_rope(const float* table, int S, int hd, int cols, const void* bias) {
-  b200::g_rope_table = table; b200::g_rope_S = S; b200::g_rope_hd = hd; b200::g_rope_cols = cols;
-  b200::g_rope_bias = static_cast<const __nv_bfloat16*>(bias);
-}
-
-// world > 1: rotate the tile raster by rank * tiles / world (0 / 1 = no rotation).  bulk = 1: tiles are staged in shared
-// memory and leave as 128-byte cp.async.bulk stores; 0: 4-byte stores straight from the accumulator registers.
-extern "C" void b200_gemm2_set_push(void* const* bases, long long n, long long off, int rank, int bulk, int world) {
-  b200::g_push_bases = bases; b200::g_push_n = n; b200::g_push_off = off; b200::g_push_rank = rank;
-  b200::g_push_bulk = bulk ? 1 : 0;
-  b200::g_push_world = world < 1 ? 1 : world;
-}
-
-extern "C" void b200_gemm2_set_swiglu(void* aux, int ld_aux, int F, int gate_first) {
-  b200::g_swi_aux = aux; b200::g_swi_ld = ld_aux; b200::g_swi_F = F; b200::g_swi_gate_first = gate_first;
-}
 
 // tile of the single-GPU GEMMs: 0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256 where the epilogue allows it
 extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode == 1 || mode == 2) ? mode : 0; }
@@ -796,46 +788,28 @@ extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode ==
 // stored [K,N] (N contiguous) else [N,K].  lda/ldb/ldc/ldr are row strides in elements.  Returns 0 or an error code.
 extern "C" int b200_gemm2_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda,
                                int ldb, int ldc, int ldr, int a_mn, int b_mn, int epi, int out_fp32,
-                               cudaStream_t stream) {
+                               const GemmEpilogueArgs& ea, cudaStream_t stream) {
   using namespace b200;
   CUtensorMap tmA, tmB;
   if (int rc = make_maps(&tmA, &tmB, A, B, M, N, K, lda, ldb, a_mn, b_mn)) return rc;
-  GemmParams p = make_params(C, R, M, N, K, ldc, ldr, epi);
-  if (epi == EPI_SWIGLU) {   // nt; N = 2F rows of the fused weight, tiles of 64 features
-    if (a_mn || b_mn || out_fp32 || !p.aux || p.swi_F <= 0 || N != 2 * p.swi_F || (p.swi_F % 64) || (p.ld_aux % 8)) return -11;
+  if (int rc = check_epilogue(ea, epi, N, ldc, a_mn, b_mn, out_fp32)) return rc;
+  GemmParams p = make_params(C, R, M, N, K, ldc, ldr, epi, ea);
+  if (epi == EPI_SWIGLU) {
     p.N = p.swi_F;
     p.n_tiles = p.swi_F / 64;
     return launch_local<false, false, EPI_SWIGLU, __nv_bfloat16>(tmA, tmB, p, stream);
   }
-  if (epi == EPI_SWIGLU_BWD) {   // nn; N = F columns of dS, output [M, 2F]
-    if (a_mn || !b_mn || out_fp32 || !p.aux || p.swi_F != N || (N % 8) || (p.ld_aux % 8)) return -12;
-    return launch_local<false, true, EPI_SWIGLU_BWD, __nv_bfloat16>(tmA, tmB, p, stream);
-  }
-  if (epi == EPI_ROPE || epi == EPI_ROPE_BIAS) {
-    if (a_mn || b_mn || out_fp32 || !p.rope || (p.rope_hd % 8) || (p.rope_cols % 8)) return -8;
-    if (epi == EPI_ROPE) return launch_local<false, false, EPI_ROPE, __nv_bfloat16>(tmA, tmB, p, stream);
-    if (!p.bias) return -8;
-    return launch_local<false, false, EPI_ROPE_BIAS, __nv_bfloat16>(tmA, tmB, p, stream);
-  }
-  if (epi == EPI_PUSH) {   // wgrad (tn) only; every 8-element vector must stay inside one owner's slice
-    if (!a_mn || !b_mn || out_fp32 || !p.push_bases || p.push_n <= 0 || (p.push_n % 8) || (p.push_off % 8) || (ldc % 8))
-      return -9;
-    return launch<true, true, EPI_PUSH, __nv_bfloat16, false>(tmA, tmB, p, AgParams{}, stream);
-  }
+  if (epi == EPI_SWIGLU_BWD) return launch_local<false, true, EPI_SWIGLU_BWD, __nv_bfloat16>(tmA, tmB, p, stream);
+  if (epi == EPI_ROPE) return launch_local<false, false, EPI_ROPE, __nv_bfloat16>(tmA, tmB, p, stream);
+  if (epi == EPI_ROPE_BIAS) return launch_local<false, false, EPI_ROPE_BIAS, __nv_bfloat16>(tmA, tmB, p, stream);
+  if (epi == EPI_PUSH) return launch<true, true, EPI_PUSH, __nv_bfloat16, false>(tmA, tmB, p, AgParams{}, stream);
+  if (epi < EPI_STORE || epi > EPI_ACCUM) return -10;
   if (a_mn) {
     if (b_mn) return dispatch_epi<true, true>(tmA, tmB, p, epi, out_fp32, stream);
     return dispatch_epi<true, false>(tmA, tmB, p, epi, out_fp32, stream);
   }
   if (b_mn) return dispatch_epi<false, true>(tmA, tmB, p, epi, out_fp32, stream);
   return dispatch_epi<false, false>(tmA, tmB, p, epi, out_fp32, stream);
-}
-
-// store / residual / accumulate epilogues only (the small-M path of the bindings)
-extern "C" int b200_gemm_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda,
-                              int ldb, int ldc, int ldr, int a_mn, int b_mn, int epi, int out_fp32,
-                              cudaStream_t stream) {
-  if (epi < 0 || epi > 2) return -10;
-  return b200_gemm2_bf16(A, B, C, R, M, N, K, lda, ldb, ldc, ldr, a_mn, b_mn, epi, out_fp32, stream);
 }
 
 // Batched C[b0,b1] = op(A[b0,b1]) op(B[b0,b1]) (+C): nb0 x nb1 problems of identical shape; sa*/sb*/sc* are the element
@@ -877,7 +851,7 @@ extern "C" int b200_bgemm_bf16(const void* A, const void* B, void* C, int M, int
 //                  contiguous.  epi store or accumulate, bf16 or fp32 output.
 extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, const int* tile, const int* seg, int E,
                                       int Mpad, int M, int N, int K, int lda, int ldb, int ldc, int layout, int epi,
-                                      int out_fp32, cudaStream_t stream) {
+                                      int out_fp32, const GemmEpilogueArgs& ea, cudaStream_t stream) {
   using namespace b200;
   if (E < 1 || Mpad % BM || (N % 8) || (K % 8) || (M % 8)) return -14;
   CUtensorMap tmA, tmB;
@@ -886,7 +860,7 @@ extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, con
     if (epi != EPI_STORE && epi != EPI_ACCUM) return -14;
     if (make_tmap_2d_bf16(&tmA, A, (uint64_t)M, (uint64_t)Mpad, (uint64_t)lda, 64, BK)) return 1001;
     if (make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)Mpad, (uint64_t)ldb, 64, BK)) return 2001;
-    GemmParams p = make_params(C, nullptr, M, N, Mpad, ldc, 0, epi);
+    GemmParams p = make_params(C, nullptr, M, N, Mpad, ldc, 0, epi, ea);
     p.nb0 = E; p.nb1 = 1; p.sc0 = (long long)M * N; p.sc1 = 0;
     p.grp_seg = seg;
     constexpr int G = GRP_K;
@@ -899,14 +873,14 @@ extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, con
   }
   if (out_fp32 || M != Mpad) return -14;
   if (make_tmap_2d_bf16(&tmA, A, (uint64_t)K, (uint64_t)Mpad, (uint64_t)lda, BK, BM)) return 1001;
-  GemmParams p = make_params(C, nullptr, Mpad, N, K, ldc, 0, epi);
+  GemmParams p = make_params(C, nullptr, Mpad, N, K, ldc, 0, epi, ea);
   p.grp_tile = tile;
   constexpr int G = GRP_M;
   if (layout == 0) {
     if (make_tmap_2d_bf16(&tmB, B, (uint64_t)K, (uint64_t)E * N, (uint64_t)ldb, BK, 64)) return 2001;
     p.grp_rows = N;
     if (epi == EPI_SWIGLU) {
-      if (!p.aux || p.swi_F <= 0 || N != 2 * p.swi_F || (p.swi_F % 64) || (p.ld_aux % 8)) return -11;
+      if (int rc = check_epilogue(ea, epi, N, ldc, 0, 0, 0)) return rc;   // nt, bf16 output
       p.N = p.swi_F;
       p.n_tiles = p.swi_F / 64;
       return launch<false, false, G | EPI_SWIGLU, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
@@ -918,7 +892,7 @@ extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, con
   if (make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)E * K, (uint64_t)ldb, 64, BK)) return 2001;
   p.grp_rows = K;
   if (epi == EPI_SWIGLU_BWD) {
-    if (!p.aux || p.swi_F != N || (p.ld_aux % 8)) return -12;
+    if (int rc = check_epilogue(ea, epi, N, ldc, 0, 1, 0)) return rc;   // nn, bf16 output
     return launch<false, true, G | EPI_SWIGLU_BWD, __nv_bfloat16, false>(tmA, tmB, p, ag, stream);
   }
   if (epi != EPI_STORE) return -14;
@@ -928,7 +902,7 @@ extern "C" int b200_gemm_grouped_bf16(const void* A, const void* B, void* C, con
 // GEMM + fused all-gather.  Supported: bf16 output, EPI store|residual|rope|rope_bias|swiglu (nt), store|residual|swiglu_bwd (nn),
 // store|accumulate|push (tn).
 extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const void* R, int M, int N, int K, int lda,
-                                  int ldb, int ldc, int ldr, int a_mn, int b_mn, int epi,
+                                  int ldb, int ldc, int ldr, int a_mn, int b_mn, int epi, const GemmEpilogueArgs& ea,
                                   const void* const* peer_shards, void* full, unsigned long long shard_bytes,
                                   unsigned long long begin, unsigned long long end, int world, int rank,
                                   uint32_t* flags, uint32_t epoch, int dependent, cudaStream_t stream) {
@@ -936,13 +910,14 @@ extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const v
   if ((begin % 16) || (end % 16) || (begin % AG_CHUNK)) return -5;
   CUtensorMap tmA, tmB;
   if (int rc = make_maps(&tmA, &tmB, A, B, M, N, K, lda, ldb, a_mn, b_mn)) return rc;
-  GemmParams p = make_params(C, R, M, N, K, ldc, ldr, epi);
+  // a dependent launch waits for B rows [n0, n0 + 128) only, but a SwiGLU tile also reads rows n0 + F
+  if (epi == EPI_SWIGLU && dependent) return -11;
+  if (int rc = check_epilogue(ea, epi, N, ldc, a_mn, b_mn, 0)) return rc;
+  GemmParams p = make_params(C, R, M, N, K, ldc, ldr, epi, ea);
   if (epi == EPI_SWIGLU) {
-    if (a_mn || b_mn || !p.aux || p.swi_F <= 0 || N != 2 * p.swi_F || (p.swi_F % 64) || (p.ld_aux % 8) || dependent) return -11;
     p.N = p.swi_F;
     p.n_tiles = p.swi_F / 64;
   }
-  if (epi == EPI_SWIGLU_BWD && (a_mn || !b_mn || !p.aux || p.swi_F != N || (N % 8) || (p.ld_aux % 8))) return -12;
   AgParams ag;
   ag.peer_shards = peer_shards; ag.full = (uint8_t*)full; ag.shard_bytes = shard_bytes; ag.begin = begin; ag.end = end;
   ag.world = world; ag.rank = rank; ag.flags = flags; ag.epoch = epoch; ag.dependent = dependent;
@@ -950,12 +925,8 @@ extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const v
   ag.b_row_bytes = (unsigned long long)ldb * 2;
   if (dependent && ((const uint8_t*)B < (const uint8_t*)full)) return -6;
 #define AGL(AM, BM_, E) return launch<AM, BM_, E, __nv_bfloat16, true>(tmA, tmB, p, ag, stream)
-  if (epi == EPI_ROPE || epi == EPI_ROPE_BIAS) {
-    if (a_mn || b_mn || !p.rope || (p.rope_hd % 8) || (p.rope_cols % 8)) return -8;
-    if (epi == EPI_ROPE) AGL(false, false, EPI_ROPE);
-    if (!p.bias) return -8;
-    AGL(false, false, EPI_ROPE_BIAS);
-  }
+  if (epi == EPI_ROPE) AGL(false, false, EPI_ROPE);
+  if (epi == EPI_ROPE_BIAS) AGL(false, false, EPI_ROPE_BIAS);
   if (!a_mn && !b_mn) {
     if (epi == EPI_SWIGLU) AGL(false, false, EPI_SWIGLU);
     if (epi == EPI_RESIDUAL) AGL(false, false, EPI_RESIDUAL);
@@ -967,10 +938,8 @@ extern "C" int b200_gemm2_ag_bf16(const void* A, const void* B, void* C, const v
     AGL(false, true, EPI_STORE);
   }
   if (a_mn && b_mn) {
-    if (epi == EPI_PUSH) {   // wgrad that pushes its tiles to the owners AND carries the next unit's all-gather
-      if (!p.push_bases || p.push_n <= 0 || (p.push_n % 8) || (p.push_off % 8) || (ldc % 8)) return -9;
-      AGL(true, true, EPI_PUSH);
-    }
+    // wgrad that pushes its tiles to the owners AND carries the next unit's all-gather
+    if (epi == EPI_PUSH) AGL(true, true, EPI_PUSH);
     if (epi == EPI_ACCUM) AGL(true, true, EPI_ACCUM);
     AGL(true, true, EPI_STORE);
   }

@@ -19,7 +19,9 @@ _LAYOUT = {"nt": 0, "nn": 1, "tn": 2}
 # attention implementation: "wgmma" (ours) | "sdpa" (library fallback, debugging only)
 ATTN_IMPL = os.environ.get("FMS_B200_ATTN_IMPL", "wgmma")
 GEMM_IMPL = os.environ.get("FMS_B200_GEMM_IMPL", "wgmma")  # "cublas" = library fallback, debugging only
-_C.set_gemm_2cta(os.environ.get("FMS_B200_GEMM_2CTA", "1") == "1")  # fused-epilogue GEMM paths (RoPE, SwiGLU, push, fp8) for M >= 256
+# The fused GEMM epilogues (RoPE, SwiGLU, push) and the fused all-gather run on GEMMs with at least this many rows (the
+# bindings refuse fewer); smaller GEMMs take the unfused paths.
+FUSED_EPI_MIN_ROWS = 256
 
 
 def launch_count() -> int:
@@ -94,12 +96,13 @@ def flush_ag_request(req=None):
                 _standalone_gather(r)
 
 
-def _try_fused_gather(a, b, layout, out, epi, residual) -> bool:
+def _try_fused_gather(a, b, layout, out, epi, residual, **epi_args) -> bool:
+    """``epi_args``: the fused epilogue's operands, passed on to ``_C.gemm_ag``."""
     if not _AG_QUEUE:
         return False
     req = _AG_QUEUE[0]
     M = a.shape[1] if layout == "tn" else a.shape[0]
-    ok = (M >= 256 and out.dtype == torch.bfloat16 and _C.get_gemm_2cta()
+    ok = (M >= FUSED_EPI_MIN_ROWS and out.dtype == torch.bfloat16
           and ((layout in ("nt", "nn") and epi in (0, 1)) or (layout == "tn" and epi in (0, 2, 4))
                or (layout == "nt" and epi == 5 and not req["dependent"]) or (layout == "nn" and epi == 6)
                or (layout == "nt" and epi in (3, 8))))
@@ -120,7 +123,7 @@ def _try_fused_gather(a, b, layout, out, epi, residual) -> bool:
         take = max(_AG_CHUNK, (take + _AG_CHUNK - 1) // _AG_CHUNK * _AG_CHUNK)
         hi = min(end, begin + take)
     _C.gemm_ag(a, b, None if epi == 4 else out, _LAYOUT[layout], epi, residual, req["table"], req["full"], req["shard_bytes"], begin,
-               hi, req["world"], req["rank"], req["flags"], req["epoch"], bool(req["dependent"]))
+               hi, req["world"], req["rank"], req["flags"], req["epoch"], bool(req["dependent"]), **epi_args)
     AG_STATS["carrier_gemms"] += 1
     if hi >= end:
         _AG_QUEUE.pop(0)
@@ -158,22 +161,23 @@ PUSH_STATS = {"gemms": 0, "with_gather": 0}
 
 def push_eligible_shape(shape) -> bool:
     """Weight shapes the push epilogue handles (wgrad GEMM, 8-element vectors never straddle an owner)."""
-    return len(shape) == 2 and shape[0] >= 256 and shape[0] % 8 == 0 and shape[1] % 8 == 0
+    return len(shape) == 2 and shape[0] >= FUSED_EPI_MIN_ROWS and shape[0] % 8 == 0 and shape[1] % 8 == 0
 
 
 def _gemm_push(a, b, tgt: PushTarget):
     M, N = a.shape[1], b.shape[1]
     if (a.dtype != torch.bfloat16 or b.dtype != torch.bfloat16 or (M, N) != tgt.shape or not push_eligible_shape((M, N))
-            or not _C.get_gemm_2cta() or a.shape[0] % 8):
+            or a.shape[0] % 8):
         raise RuntimeError(f"wgrad {tuple(a.shape)}^T x {tuple(b.shape)} cannot use the push epilogue")
     a = a if a.stride(-1) == 1 else a.contiguous()
     b = b if b.stride(-1) == 1 else b.contiguous()
-    _C.set_gemm_push(tgt.table, tgt.n, tgt.off, tgt.rank, PUSH_BULK, tgt.world if PUSH_ROTATE else 1)
+    push = dict(push_bases=tgt.table, push_n=tgt.n, push_off=tgt.off, push_rank=tgt.rank, push_bulk=PUSH_BULK,
+                push_world=tgt.world if PUSH_ROTATE else 1)
     PUSH_STATS["gemms"] += 1
-    if _AG_QUEUE and _try_fused_gather(a, b, "tn", tgt, 4, None):
+    if _AG_QUEUE and _try_fused_gather(a, b, "tn", tgt, 4, None, **push):
         PUSH_STATS["with_gather"] += 1      # the same kernel pushes its tiles out and pulls the next unit's weights in
         return tgt
-    _C.gemm_push(a, b)
+    _C.gemm_push(a, b, **push)
     return tgt
 
 
@@ -191,7 +195,7 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
     if rope is not None:
         M0 = a.shape[0]
         ok = (GEMM_IMPL == "wgmma" and layout == "nt" and a.dtype == b.dtype == torch.bfloat16 and residual is None
-              and not accumulate and M0 >= 256 and M0 % 8 == 0 and _C.get_gemm_2cta() and rope[2] % 8 == 0
+              and not accumulate and M0 >= FUSED_EPI_MIN_ROWS and M0 % 8 == 0 and rope[2] % 8 == 0
               and a.shape[1] % 8 == 0 and b.shape[0] % 8 == 0 and out_dtype in (None, torch.bfloat16)
               and (out is None or out.dtype == torch.bfloat16)
               and (bias is None or (bias.dtype == torch.bfloat16 and bias.is_contiguous()
@@ -220,6 +224,7 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
     if out is None:
         out = torch.empty(M, N, dtype=out_dtype or a.dtype, device=a.device)
     epi = 0
+    epi_args = {}
     if residual is not None:
         if accumulate:
             raise ValueError("residual and accumulate are mutually exclusive")
@@ -228,10 +233,11 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
         epi = 2
     if rope is not None:
         epi = 3 if bias is None else 8
-        _C.set_gemm_rope(rope[0], int(rope[1]), int(rope[2]), int((rope[3] + rope[4]) * rope[2]), bias)   # for the launch below
-    if _AG_QUEUE and _try_fused_gather(a, b, layout, out, epi, residual):
+        epi_args = dict(rope_table=rope[0], rope_S=int(rope[1]), rope_hd=int(rope[2]),
+                        rope_cols=int((rope[3] + rope[4]) * rope[2]), bias=bias)
+    if _AG_QUEUE and _try_fused_gather(a, b, layout, out, epi, residual, **epi_args):
         return out
-    _C.gemm(a, b, out, _LAYOUT[layout], epi, residual)
+    _C.gemm(a, b, out, _LAYOUT[layout], epi, residual, **epi_args)
     return out
 
 
@@ -243,8 +249,8 @@ FUSE_SWIGLU_BWD = os.environ.get("FMS_B200_FUSE_SWIGLU_BWD", "1") == "1"
 
 
 def _swiglu_fusable(x, F):
-    return (FUSE_SWIGLU and GEMM_IMPL == "wgmma" and x.dtype == torch.bfloat16 and x.shape[0] >= 256 and x.shape[0] % 8 == 0
-            and _C.get_gemm_2cta())
+    return (FUSE_SWIGLU and GEMM_IMPL == "wgmma" and x.dtype == torch.bfloat16 and x.shape[0] >= FUSED_EPI_MIN_ROWS
+            and x.shape[0] % 8 == 0)
 
 
 def gated_up_fwd(x, w, gate_first=True):
@@ -258,10 +264,10 @@ def gated_up_fwd(x, w, gate_first=True):
     w = w if w.stride(-1) == 1 else w.contiguous()
     gu = torch.empty(x.shape[0], 2 * F, dtype=torch.bfloat16, device=x.device)
     act = torch.empty(x.shape[0], F, dtype=torch.bfloat16, device=x.device)
-    _C.set_gemm_swiglu(act, F, bool(gate_first))
-    if _AG_QUEUE and _try_fused_gather(x, w, "nt", gu, 5, None):
+    swiglu = dict(aux=act, swiglu_F=F, gate_first=bool(gate_first))
+    if _AG_QUEUE and _try_fused_gather(x, w, "nt", gu, 5, None, **swiglu):
         return gu, act
-    _C.gemm(x, w, gu, 0, 5, None)
+    _C.gemm(x, w, gu, 0, 5, None, **swiglu)
     return gu, act
 
 
@@ -275,10 +281,10 @@ def gated_down_bwd(dy, w2, gu, gate_first=True):
     dy = dy if dy.stride(-1) == 1 else dy.contiguous()
     w2 = w2 if w2.stride(-1) == 1 else w2.contiguous()
     dgu = torch.empty_like(gu)
-    _C.set_gemm_swiglu(gu, F, bool(gate_first))
-    if _AG_QUEUE and _try_fused_gather(dy, w2, "nn", dgu, 6, None):
+    swiglu = dict(aux=gu, swiglu_F=F, gate_first=bool(gate_first))
+    if _AG_QUEUE and _try_fused_gather(dy, w2, "nn", dgu, 6, None, **swiglu):
         return dgu
-    _C.gemm(dy, w2, dgu, 1, 6, None)
+    _C.gemm(dy, w2, dgu, 1, 6, None, **swiglu)
     return dgu
 
 
@@ -324,8 +330,7 @@ def moe_up_fwd(xp, w1, plan, T, k):
     F = w1.shape[1] // 2
     h = torch.empty(xp.shape[0], 2 * F, dtype=torch.bfloat16, device=xp.device)
     s = torch.empty(xp.shape[0], F, dtype=torch.bfloat16, device=xp.device)
-    _C.set_gemm_swiglu(s, F, True)
-    _C.gemm_grouped(xp, w1.contiguous(), h, plan, int(T), int(k), 0, 5)
+    _C.gemm_grouped(xp, w1.contiguous(), h, plan, int(T), int(k), 0, 5, aux=s, swiglu_F=F, gate_first=True)
     return h, s
 
 
@@ -337,8 +342,7 @@ def moe_down_fwd(sp, w2, plan, T, k):
 
 def moe_down_bwd(dyp, w2, hp, plan, T, k):
     dh = torch.empty_like(hp)
-    _C.set_gemm_swiglu(hp, w2.shape[2], True)
-    _C.gemm_grouped(dyp, w2.contiguous(), dh, plan, int(T), int(k), 1, 6)
+    _C.gemm_grouped(dyp, w2.contiguous(), dh, plan, int(T), int(k), 1, 6, aux=hp, swiglu_F=w2.shape[2], gate_first=True)
     return dh
 
 
@@ -367,7 +371,7 @@ def gemm_fp8(aq, bq, sa, sb, out=None):
     N = bq.shape[0]
     if out is None:
         out = torch.empty(M, N, dtype=torch.bfloat16, device=aq.device)
-    if K % 16 or N % 8 or not _C.get_gemm_2cta():
+    if K % 16 or N % 8:
         return _fallback("gemm_fp8").gemm_fp8(aq, bq, sa, sb, out)
     _C.gemm_fp8(aq, bq, sa, sb, out)
     return out

@@ -122,8 +122,8 @@ if mode in ("all", "push"):
         staging.zero_()
         fc.shard.barrier(C, fc._anchor)
         def push():
-            C.set_gemm_push(table, n, 0, rank, bulk, world if rotate else 1)
-            C.gemm_push(dy, x)                           # layout tn, push epilogue
+            C.gemm_push(dy, x, push_bases=table, push_n=n, push_off=0, push_rank=rank, push_bulk=bulk,
+                        push_world=world if rotate else 1)   # layout tn, push epilogue
         push()
         fc.shard.barrier(C, fc._anchor)                  # every rank's tiles have landed in my slots
         C.reduce_scatter(slots, mine, 0, world, 0, True, 1.0, None)     # local 'world'-way sum of the slots

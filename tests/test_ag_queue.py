@@ -14,10 +14,8 @@ class _Rec:
     def __init__(self):
         self.ag, self.plain = [], []
 
-    def get_gemm_2cta(self):
-        return True
-
-    def gemm_ag(self, a, b, out, layout, epi, residual, table, full, shard_bytes, begin, end, world, rank, flags, epoch, dep):
+    def gemm_ag(self, a, b, out, layout, epi, residual, table, full, shard_bytes, begin, end, world, rank, flags, epoch, dep,
+                **epi_args):
         self.ag.append((begin, end, bool(dep)))
 
     def p2p_gather_range(self, table, full, shard_bytes, begin, end):

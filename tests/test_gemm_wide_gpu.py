@@ -90,8 +90,7 @@ def make_case(CK, TK, layout, M, N, Kd, epi, odt, seed):
         def run():   # the launcher itself, so that an F the wide tile cannot take reaches it
             gu = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
             act = torch.empty(M, Fh, dtype=torch.bfloat16, device=DEV)
-            CK._C.set_gemm_swiglu(act, Fh, True)
-            CK._C.gemm(x, w, gu, 0, 5, None)
+            CK._C.gemm(x, w, gu, 0, 5, None, aux=act, swiglu_F=Fh, gate_first=True)
             return gu, act
         return run, (gu0, None)
     if epi == "swiglu_bwd":

@@ -170,8 +170,8 @@ def test_wgrad_push_epilogue_then_slot_sum_is_reduce_scatter(C, shape, bulk):
     for r in range(W):
         dy = (torch.randn(T, Nw, device=DEV) * 0.1).bfloat16()
         x = (torch.randn(T, Kd, device=DEV) * 0.1).bfloat16()
-        C.set_gemm_push(tab, n, off, r, bulk, W if Nw != 512 else 1)   # rank-rotated tile raster (and one case without)
-        C.gemm_push(dy, x)
+        C.gemm_push(dy, x, push_bases=tab, push_n=n, push_off=off, push_rank=r, push_bulk=bulk,
+                    push_world=W if Nw != 512 else 1)   # rank-rotated tile raster (and one case without)
         ref[off:off + Nw * Kd] += (dy.float().t() @ x.float()).bfloat16().float().reshape(-1)
     torch.cuda.synchronize()
     for o in range(W):

@@ -68,8 +68,7 @@ def test_push_epilogue_slot_sum_accumulates_over_micro_steps(C):
         for r in range(W):
             dy = (torch.randn(T, Nw, device=DEV) * 0.1).bfloat16()
             x = (torch.randn(T, Kd, device=DEV) * 0.1).bfloat16()
-            C.set_gemm_push(tab, n, off, r, True, W)
-            C.gemm_push(dy, x)
+            C.gemm_push(dy, x, push_bases=tab, push_n=n, push_off=off, push_rank=r, push_bulk=True, push_world=W)
             ref[off:off + Nw * Kd] += (dy.float().t() @ x.float()).bfloat16().float().reshape(-1)
         torch.cuda.synchronize()
         for o in range(W):

@@ -117,8 +117,8 @@ def test_fused_all_gather_build_gives_the_same_bits(K, dependent):
         flags = torch.zeros((total * 2 + 65535) // 65536, dtype=torch.int32, device=DEV)
         wm = (full if dependent else flat)[:N * D].view(N, D)
         y = torch.empty(B * S, N, dtype=torch.bfloat16, device=DEV)
-        CK._C.set_gemm_rope(table, S, hd, (H + KVH) * hd, b)
-        CK._C.gemm_ag(x, wm, y, 0, 8, None, _table(shards), full, n * 2, 0, total * 2, W, r, flags, 1, dependent)
+        CK._C.gemm_ag(x, wm, y, 0, 8, None, _table(shards), full, n * 2, 0, total * 2, W, r, flags, 1, dependent,
+                      rope_table=table, rope_S=S, rope_hd=hd, rope_cols=(H + KVH) * hd, bias=b)
         torch.cuda.synchronize()
         assert torch.equal(full, flat)
         assert torch.equal(y, want)
