@@ -58,7 +58,9 @@ DECL int b200_qk_norm_bwd(void*, const void*, const float*, const void*, const v
 DECL int b200_swiglu_fwd(const void*, void*, long long, int, int, cudaStream_t);
 DECL int b200_swiglu_bwd(const void*, const void*, void*, long long, int, int, cudaStream_t);
 DECL int b200_embedding_fwd(const void*, int, const void*, void*, long long, int, cudaStream_t);
-DECL int b200_embedding_bwd(const void*, int, const void*, void*, int, long long, int, cudaStream_t);
+DECL int b200_embedding_bwd_chunks(long long);
+DECL int b200_embedding_bwd(const void*, int, const void*, void*, int, long long, int, unsigned long long*, float*, int*,
+                            cudaStream_t);
 DECL int b200_count_valid(const long long*, int, long long, float*, cudaStream_t);
 DECL int b200_ce_grad_inplace(void*, const long long*, const float*, float*, int, int, int, long long, cudaStream_t);
 DECL int b200_adamw(float*, const void*, int, float*, float*, void*, long long, float, float, float, float, float,
@@ -416,15 +418,23 @@ at::Tensor embedding_fwd(const at::Tensor& tok, const at::Tensor& w) {
                            cur_stream()), "embedding_fwd");
   return out;
 }
+// dw [V, D] += the rows of dx at tok, each row of dw summed in fp32 and rounded once, in a fixed order
 void embedding_bwd(const at::Tensor& dx, const at::Tensor& tok, at::Tensor& dw) {
   c10::cuda::CUDAGuard guard(dx.device());
   need(dx, "dx", at::kBFloat16);
   TORCH_CHECK(dx.is_contiguous() && tok.is_contiguous() && dw.is_contiguous());
+  TORCH_CHECK(tok.is_cuda() && (tok.scalar_type() == at::kLong || tok.scalar_type() == at::kInt), "embedding_bwd: tokens");
   TORCH_CHECK(dw.scalar_type() == at::kBFloat16 || dw.scalar_type() == at::kFloat);
   const int D = dx.size(-1);
   const int64_t M = tok.numel();
-  check(b200_embedding_bwd(tok.data_ptr(), tok.scalar_type() == at::kLong, dx.data_ptr(), dw.data_ptr(),
-                           dw.scalar_type() == at::kFloat, M, D, cur_stream()), "embedding_bwd");
+  TORCH_CHECK(dw.dim() == 2 && dw.size(1) == D && dx.numel() == M * D, "embedding_bwd: shapes");
+  auto keys = at::empty({2 * M}, tok.options().dtype(at::kLong));
+  auto part = at::empty({2 * (int64_t)b200_embedding_bwd_chunks(M), D}, dx.options().dtype(at::kFloat));
+  int launches = 0;
+  const int rc = b200_embedding_bwd(tok.data_ptr(), tok.scalar_type() == at::kLong, dx.data_ptr(), dw.data_ptr(),
+                                    dw.scalar_type() == at::kFloat, M, D, (unsigned long long*)keys.data_ptr(),
+                                    part.data_ptr<float>(), &launches, cur_stream());
+  check(rc, "embedding_bwd", launches);
 }
 void count_valid(const at::Tensor& labels, int64_t ignore, at::Tensor& n_valid) {
   c10::cuda::CUDAGuard guard(labels.device());

@@ -555,29 +555,176 @@ __global__ void embedding_fwd_kernel(const IdxT* __restrict__ tok, const __nv_bf
     *reinterpret_cast<uint4*>(out + row * D + c) = *reinterpret_cast<const uint4*>(w + t * D + c);
   }
 }
+// Backward: dw[t] = round(dw[t] + sum of dx[i] over the positions i with tok[i] == t), each row summed in fp32 in
+// position order and rounded once; no float atomics, so two runs give the same bits.
+//   1. sort the keys (tok[i] << 32 | i): they are unique, so the sorted order does not depend on how it was reached.
+//      embedding_sort_tile_kernel sorts tiles of EMB_TILE keys in shared memory (bitonic), embedding_merge_kernel
+//      merges pairs of sorted runs (every key finds its place by a binary search in the partner run), log2(M / EMB_TILE)
+//      times.  Equal tokens end up adjacent, in position order.
+//   2. embedding_seg_sum_kernel: chunk c of EMB_CHUNK sorted keys sums each run of equal tokens it holds.  A run inside
+//      the chunk is written to dw; the chunk's first and last runs, when they continue into a neighbouring chunk, go to
+//      part[c][0] and part[c][1].  embedding_seg_combine_kernel: the chunk where such a run starts adds the partial sums
+//      of the chunks it covers in chunk order and writes the row.  A token repeated M times costs M / EMB_CHUNK adds.
+constexpr int EMB_TILE = 4096, EMB_SORT_NT = 512, EMB_CHUNK = 64, EMB_COLS = 2048;   // EMB_COLS columns per CTA
+
+B200_DEVINL unsigned emb_tok(unsigned long long k) { return (unsigned)(k >> 32); }
+
 template <typename IdxT>
-__global__ void embedding_bwd_kernel(const IdxT* __restrict__ tok, const __nv_bfloat16* __restrict__ dx,
-                                     __nv_bfloat16* __restrict__ dw, size_t M, int D) {
-  const int vec = D / 2;
-  const size_t total = M * vec;
-  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (size_t)gridDim.x * blockDim.x) {
-    const size_t row = idx / vec;
-    const int c = (int)(idx % vec) * 2;
-    const size_t t = (size_t)tok[row];
-    const __nv_bfloat162 v = *reinterpret_cast<const __nv_bfloat162*>(dx + row * D + c);
-    atomicAdd(reinterpret_cast<__nv_bfloat162*>(dw + t * D + c), v);
+__global__ void __launch_bounds__(EMB_SORT_NT) embedding_sort_tile_kernel(const IdxT* __restrict__ tok,
+                                                                         unsigned long long* __restrict__ keys, int M) {
+  __shared__ unsigned long long s[EMB_TILE];
+  const int base = blockIdx.x * EMB_TILE;
+  for (int i = threadIdx.x; i < EMB_TILE; i += EMB_SORT_NT) {
+    const int g = base + i;
+    s[i] = g < M ? ((unsigned long long)(unsigned)tok[g] << 32) | (unsigned)g : ~0ull;   // padding sorts last
   }
+  __syncthreads();
+  for (int k = 2; k <= EMB_TILE; k <<= 1) {
+    for (int j = k >> 1; j > 0; j >>= 1) {
+      for (int p = threadIdx.x; p < EMB_TILE / 2; p += EMB_SORT_NT) {
+        const int i = ((p & ~(j - 1)) << 1) | (p & (j - 1)), l = i + j;
+        const unsigned long long a = s[i], b = s[l];
+        if ((a > b) == ((i & k) == 0)) {
+          s[i] = b;
+          s[l] = a;
+        }
+      }
+      __syncthreads();
+    }
+  }
+  for (int i = threadIdx.x; i < EMB_TILE; i += EMB_SORT_NT)
+    if (base + i < M) keys[base + i] = s[i];
 }
-template <typename IdxT>
-__global__ void embedding_bwd_f32_kernel(const IdxT* __restrict__ tok, const __nv_bfloat16* __restrict__ dx,
-                                         float* __restrict__ dw, size_t M, int D) {
-  const size_t total = M * D;
-  for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (size_t)gridDim.x * blockDim.x) {
-    const size_t row = idx / D;
-    const int c = (int)(idx % D);
-    atomicAdd(dw + (size_t)tok[row] * D + c, __bfloat162float(dx[idx]));
+
+// runs [2rL, 2rL + L) and [2rL + L, 2rL + 2L) of `in` (clipped to M) -> one sorted run of `out`
+__global__ void __launch_bounds__(256) embedding_merge_kernel(const unsigned long long* __restrict__ in,
+                                                              unsigned long long* __restrict__ out, int M, int L) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M) return;
+  const unsigned long long key = in[i];
+  const int r = i / L, own = i - r * L;
+  const int first = (r & 1) ? (r - 1) * L : r * L;             // start of the merged run
+  int lo = (r & 1) ? (r - 1) * L : (r + 1) * L;                  // the partner run [lo, hi)
+  int hi = min(M, lo + L);
+  if (lo > hi) lo = hi;
+  const int p0 = lo;
+  while (lo < hi) {                                              // keys of the partner run below ours
+    const int mid = (lo + hi) >> 1;
+    if (in[mid] < key) lo = mid + 1; else hi = mid;
+  }
+  out[first + own + (lo - p0)] = key;
+}
+
+B200_DEVINL void emb_load_pair(const __nv_bfloat16* p, float& a, float& b) {
+  const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(p));
+  a = f.x;
+  b = f.y;
+}
+B200_DEVINL void emb_store_pair(__nv_bfloat16* p, float a, float b) {
+  float x, y;
+  emb_load_pair(p, x, y);
+  *reinterpret_cast<__nv_bfloat162*>(p) = __floats2bfloat162_rn(x + a, y + b);
+}
+B200_DEVINL void emb_store_pair(float* p, float a, float b) {
+  const float2 o = *reinterpret_cast<const float2*>(p);
+  *reinterpret_cast<float2*>(p) = make_float2(o.x + a, o.y + b);
+}
+
+// Lane l of the CTA owns the column pairs blockIdx.y * EMB_COLS / 2 + k * 256 + l, k = 0..3.
+template <typename OutT>
+__global__ void __launch_bounds__(256) embedding_seg_sum_kernel(const unsigned long long* __restrict__ keys,
+                                                                const __nv_bfloat16* __restrict__ dx,
+                                                                OutT* __restrict__ dw, float* __restrict__ part, int M,
+                                                                int D) {
+  __shared__ unsigned long long sk[EMB_CHUNK];
+  const int c = blockIdx.x, i0 = c * EMB_CHUNK, n = min(M - i0, EMB_CHUNK);
+  if (threadIdx.x < n) sk[threadIdx.x] = keys[i0 + threadIdx.x];
+  __syncthreads();
+  const unsigned before = i0 > 0 ? emb_tok(keys[i0 - 1]) : 0xffffffffu;
+  const unsigned after = i0 + n < M ? emb_tok(keys[i0 + n]) : 0xffffffffu;
+  int col[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) col[k] = (blockIdx.y * (EMB_COLS / 2) + k * 256 + threadIdx.x) * 2;
+  float acc[8];
+#pragma unroll
+  for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+  unsigned cur = emb_tok(sk[0]);
+  int seg = 0, start = 0;                                        // segment index in the chunk, its first key
+  auto flush = [&](int end) {
+    const bool open = (start == 0 && cur == before) || (end == n && cur == after);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (col[k] < D) {
+        if (open) {
+          *reinterpret_cast<float2*>(part + ((size_t)c * 2 + (seg == 0 ? 0 : 1)) * D + col[k]) =
+              make_float2(acc[2 * k], acc[2 * k + 1]);
+        } else {
+          emb_store_pair(dw + (size_t)cur * D + col[k], acc[2 * k], acc[2 * k + 1]);
+        }
+      }
+    }
+  };
+  for (int i = 0; i < n; i += 4) {
+    float v[4][8];                                               // four rows in flight
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const __nv_bfloat16* row = dx + (size_t)(unsigned)sk[min(i + u, n - 1)] * D;
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        v[u][2 * k] = v[u][2 * k + 1] = 0.f;
+        if (i + u < n && col[k] < D) emb_load_pair(row + col[k], v[u][2 * k], v[u][2 * k + 1]);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      if (i + u < n) {
+        const unsigned t = emb_tok(sk[i + u]);
+        if (t != cur) {
+          flush(i + u);
+#pragma unroll
+          for (int q = 0; q < 8; ++q) acc[q] = 0.f;
+          cur = t;
+          ++seg;
+          start = i + u;
+        }
+#pragma unroll
+        for (int q = 0; q < 8; ++q) acc[q] += v[u][q];
+      }
+    }
+  }
+  flush(n);
+}
+
+// One CTA per chunk c (and column block): if the run holding chunk c's last key starts in chunk c and continues past
+// it, sum its partial sums in chunk order and write the row.
+template <typename OutT>
+__global__ void __launch_bounds__(256) embedding_seg_combine_kernel(const unsigned long long* __restrict__ keys,
+                                                                    const float* __restrict__ part,
+                                                                    OutT* __restrict__ dw, int M, int D) {
+  const int c = blockIdx.x, i0 = c * EMB_CHUNK, last = i0 + EMB_CHUNK - 1;
+  if (last + 1 >= M) return;
+  const unsigned t = emb_tok(keys[last]);
+  if (emb_tok(keys[last + 1]) != t || (i0 > 0 && emb_tok(keys[i0 - 1]) == t)) return;
+  int lo = last + 1, hi = M;                                     // end of the run: first key with a larger token
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (emb_tok(keys[mid]) <= t) lo = mid + 1; else hi = mid;
+  }
+  const int c_end = (lo - 1) / EMB_CHUNK;                        // the last chunk the run reaches
+  const int slot = emb_tok(keys[i0]) == t ? 0 : 1;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int col = (blockIdx.y * (EMB_COLS / 2) + k * 256 + threadIdx.x) * 2;
+    if (col < D) {
+      float2 s = *reinterpret_cast<const float2*>(part + ((size_t)c * 2 + slot) * D + col);
+#pragma unroll 4
+      for (int c2 = c + 1; c2 <= c_end; ++c2) {
+        const float2 p = *reinterpret_cast<const float2*>(part + (size_t)c2 * 2 * D + col);
+        s.x += p.x;
+        s.y += p.y;
+      }
+      emb_store_pair(dw + (size_t)t * D + col, s.x, s.y);
+    }
   }
 }
 
@@ -994,26 +1141,37 @@ extern "C" int b200_embedding_fwd(const void* tok, int tok_is_i64, const void* w
                                                 (size_t)M, D);
   CK();
 }
+// Workspace of b200_embedding_bwd: keys [2 M] uint64 and part [2 * chunks, D] fp32.  Returns the number of chunks.
+extern "C" int b200_embedding_bwd_chunks(long long M) { return (int)((M + EMB_CHUNK - 1) / EMB_CHUNK); }
+// dw [V, D] (bf16 or fp32) += the rows of dx [M, D] (bf16) at tok [M]; *launches receives the number of kernels.
 extern "C" int b200_embedding_bwd(const void* tok, int tok_is_i64, const void* dx, void* dw, int dw_is_f32,
-                                  long long M, int D, cudaStream_t s) {
-  if (D % 2) return -1;
-  if (dw_is_f32) {
-    int g = grid_for((size_t)M * D, 256);
-    if (tok_is_i64)
-      embedding_bwd_f32_kernel<long long><<<g, 256, 0, s>>>((const long long*)tok, (const __nv_bfloat16*)dx,
-                                                            (float*)dw, (size_t)M, D);
-    else
-      embedding_bwd_f32_kernel<int><<<g, 256, 0, s>>>((const int*)tok, (const __nv_bfloat16*)dx, (float*)dw,
-                                                      (size_t)M, D);
-  } else {
-    int g = grid_for((size_t)M * (D / 2), 256);
-    if (tok_is_i64)
-      embedding_bwd_kernel<long long><<<g, 256, 0, s>>>((const long long*)tok, (const __nv_bfloat16*)dx,
-                                                        (__nv_bfloat16*)dw, (size_t)M, D);
-    else
-      embedding_bwd_kernel<int><<<g, 256, 0, s>>>((const int*)tok, (const __nv_bfloat16*)dx, (__nv_bfloat16*)dw,
-                                                  (size_t)M, D);
+                                  long long M, int D, unsigned long long* keys, float* part, int* launches,
+                                  cudaStream_t s) {
+  *launches = 0;
+  if (D % 2 || M >= (1ll << 31)) return -1;
+  if (M == 0) return 0;
+  const int m = (int)M;
+  unsigned long long *a = keys, *b = keys + M;
+  const int tiles = (m + EMB_TILE - 1) / EMB_TILE;
+  if (tok_is_i64) embedding_sort_tile_kernel<long long><<<tiles, EMB_SORT_NT, 0, s>>>((const long long*)tok, a, m);
+  else embedding_sort_tile_kernel<int><<<tiles, EMB_SORT_NT, 0, s>>>((const int*)tok, a, m);
+  int n = 1;
+  for (long long L = EMB_TILE; L < m; L *= 2, ++n) {
+    embedding_merge_kernel<<<(m + 255) / 256, 256, 0, s>>>(a, b, m, (int)L);
+    unsigned long long* t = a;
+    a = b;
+    b = t;
   }
+  const dim3 grid(b200_embedding_bwd_chunks(M), (D + EMB_COLS - 1) / EMB_COLS);
+  const __nv_bfloat16* x = (const __nv_bfloat16*)dx;
+  if (dw_is_f32) {
+    embedding_seg_sum_kernel<float><<<grid, 256, 0, s>>>(a, x, (float*)dw, part, m, D);
+    embedding_seg_combine_kernel<float><<<grid, 256, 0, s>>>(a, part, (float*)dw, m, D);
+  } else {
+    embedding_seg_sum_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(a, x, (__nv_bfloat16*)dw, part, m, D);
+    embedding_seg_combine_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>(a, part, (__nv_bfloat16*)dw, m, D);
+  }
+  *launches = n + 2;
   CK();
 }
 extern "C" int b200_count_valid(const long long* labels, int M, long long ignore, float* n_valid, cudaStream_t s) {

@@ -16,6 +16,11 @@ import torch.nn.functional as F
 NAME = "torch"
 
 
+def _f32(t):
+    """fp32 math (fp64 inputs stay fp64, so the oracle itself can be checked in double precision)."""
+    return t if t.dtype == torch.float64 else t.float()
+
+
 # ----------------------------------------------------------------------------------------------
 # GEMM family.  layout: "nt": C[M,N] = A[M,K] B[N,K]^T ; "nn": C[M,N] = A[M,K] B[K,N] ;
 #                        "tn": C[M,N] = A[K,M]^T B[K,N].  fp32 accumulate, output dtype of `out`/a.
@@ -51,20 +56,20 @@ def gemm(a, b, layout="nt", out=None, accumulate=False, residual=None, out_dtype
 # RMSNorm (fp32 math, io in x.dtype).  y = x * rsqrt(mean(x^2)+eps) * w
 # ----------------------------------------------------------------------------------------------
 def rmsnorm_fwd(x, w, eps):
-    xf = x.float()
+    xf = _f32(x)
     rstd = torch.rsqrt(xf.pow(2).mean(-1, keepdim=True) + eps)
-    y = (xf * rstd * w.float()).to(x.dtype)
+    y = (xf * rstd * _f32(w)).to(x.dtype)
     return y, rstd.squeeze(-1)
 
 
 def rmsnorm_bwd(dy, x, w, rstd, dres=None):
-    xf, dyf, wf = x.float(), dy.float(), w.float()
-    r = rstd.unsqueeze(-1)
+    xf, dyf, wf = _f32(x), _f32(dy), _f32(w)
+    r = _f32(rstd).unsqueeze(-1)
     xhat = xf * r
     g = dyf * wf
     dx = r * (g - xhat * (g * xhat).mean(-1, keepdim=True))
     if dres is not None:
-        dx = dx + dres.reshape(dx.shape).float()
+        dx = dx + _f32(dres.reshape(dx.shape))
     dw = (dyf * xhat).reshape(-1, x.shape[-1]).sum(0)
     return dx.to(x.dtype), dw
 
@@ -147,11 +152,11 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, inverse=
     if inverse:
         sin = -sin
     if interleaved:   # FMS convention: pairs (2i, 2i+1)
-        x = v.float().reshape(M, nrot, rot_dim // 2, 2)
+        x = _f32(v).reshape(M, nrot, rot_dim // 2, 2)
         x0, x1 = x[..., 0], x[..., 1]
         out = torch.stack([x0 * cos - x1 * sin, x0 * sin + x1 * cos], dim=-1).reshape(M, nrot, rot_dim)
     else:             # GPT-NeoX / HF convention: pairs (i, i + rot/2)
-        x = v.float()
+        x = _f32(v)
         x0, x1 = x[..., : rot_dim // 2], x[..., rot_dim // 2:]
         out = torch.cat([x0 * cos - x1 * sin, x0 * sin + x1 * cos], dim=-1)
     v.copy_(out.to(qkv.dtype))
@@ -164,11 +169,6 @@ def rope_(qkv, table, seq_len, nheads, kvheads, head_dim, rot_dim=None, inverse=
 # (fp32); the backward takes the gradient of the normed, UN-rotated heads (the attention backward applies the inverse
 # RoPE) and returns fp32 (dw_q, dw_k).
 # ----------------------------------------------------------------------------------------------
-def _f32(t):
-    """fp32 math (fp64 inputs stay fp64, so the oracle itself can be checked in double precision)."""
-    return t if t.dtype == torch.float64 else t.float()
-
-
 def _qk_weights(w_q, w_k, nheads, kvheads):
     return torch.cat([_f32(w_q).expand(nheads, -1), _f32(w_k).expand(kvheads, -1)])   # [H+KVH, hd]
 
@@ -311,7 +311,7 @@ def gemm_fp8(aq, bq, sa, sb, out=None):
 # ----------------------------------------------------------------------------------------------
 def swiglu_fwd(gu, gate_first=True):
     F_ = gu.shape[-1] // 2
-    a, b = gu[..., :F_].float(), gu[..., F_:].float()
+    a, b = _f32(gu[..., :F_]), _f32(gu[..., F_:])
     g, u = (a, b) if gate_first else (b, a)
     return (F.silu(g) * u).to(gu.dtype)
 
@@ -329,7 +329,7 @@ def gated_down_bwd(dy, w2, gu, gate_first=True):
 
 def swiglu_bwd(ds, gu, gate_first=True):
     F_ = gu.shape[-1] // 2
-    a, b, d = gu[..., :F_].float(), gu[..., F_:].float(), ds.float()
+    a, b, d = _f32(gu[..., :F_]), _f32(gu[..., F_:]), _f32(ds)
     g, u = (a, b) if gate_first else (b, a)
     sig = torch.sigmoid(g)
     dg = d * u * sig * (1 + g * (1 - sig))
@@ -509,9 +509,23 @@ def embedding_fwd(tokens, w):
 
 
 def embedding_bwd(dx, tokens, out, accumulate=False):
+    """out[t] = round(out[t] + sum of the rows of dx at the positions of token t): each touched row is summed in fp32
+    (fp64 for fp64 inputs) and rounded to out.dtype once.  The sums go to a [M, D] buffer, one row per distinct token
+    (its segment in the sorted token order), so nothing waits for the host to learn how many tokens are distinct."""
     if not accumulate:
         out.zero_()
-    out.index_add_(0, tokens.reshape(-1).long(), dx.to(out.dtype))
+    tok = tokens.reshape(-1).long()
+    if tok.numel() == 0:
+        return out
+    srt, order = torch.sort(tok, stable=True)
+    seg = torch.cumsum(torch.cat([srt.new_zeros(1), (srt[1:] != srt[:-1]).long()]), 0)
+    seg_of = torch.empty_like(seg)
+    seg_of[order] = seg
+    x = _f32(dx)
+    acc = torch.zeros(tok.numel(), x.shape[-1], dtype=torch.promote_types(x.dtype, out.dtype), device=x.device)
+    acc.index_add_(0, seg_of, x)
+    # every position of a token writes the same value, so repeated indices agree
+    out.index_copy_(0, tok, (out[tok].to(acc.dtype) + acc[seg_of]).to(out.dtype))
     return out
 
 
@@ -524,13 +538,14 @@ def linear_ce_fwd_bwd(h, w, labels, dw_out, ignore_index=-100, chunk_rows=4096, 
     M, D = h.shape
     labels = labels.reshape(-1).long()
     valid = labels != ignore_index
-    n_valid = valid.sum().clamp(min=1).float()
+    acc_t = _f32(h).dtype
+    n_valid = valid.sum().clamp(min=1).to(acc_t)
     dh = torch.empty_like(h)
-    loss = torch.zeros((), dtype=torch.float32, device=h.device)
+    loss = torch.zeros((), dtype=acc_t, device=h.device)
     first = not accumulate
     for s in range(0, M, chunk_rows):
         e = min(M, s + chunk_rows)
-        logits = (h[s:e] @ w.t()).float()
+        logits = _f32(h[s:e] @ w.t())
         lab = labels[s:e]
         ok = valid[s:e]
         lse = torch.logsumexp(logits, dim=-1)
@@ -550,8 +565,8 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100):
     """Unfused variant for an explicit logits tensor: returns loss and dlogits (1/n scaled)."""
     labels = labels.reshape(-1).long()
     valid = labels != ignore_index
-    n_valid = valid.sum().clamp(min=1).float()
-    lf = logits.float()
+    lf = _f32(logits)
+    n_valid = valid.sum().clamp(min=1).to(lf.dtype)
     lse = torch.logsumexp(lf, dim=-1)
     safe = labels.clamp(min=0)
     tgt = lf.gather(1, safe.unsqueeze(1)).squeeze(1)
@@ -565,7 +580,7 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100):
 # Optimizer / gradient utilities on flat shards
 # ----------------------------------------------------------------------------------------------
 def sumsq(x, out=None):
-    s = x.float().pow(2).sum()
+    s = _f32(x).pow(2).sum()
     if out is None:
         return s
     out.add_(s)
@@ -577,7 +592,7 @@ def adamw_step(master, grad, exp_avg, exp_avg_sq, lowp_out, lr, beta1, beta2, ep
     """Decoupled-weight-decay Adam on a flat fp32 shard (torch.optim.AdamW semantics).
     grad may be bf16/fp32; grad_scale is an optional 0-dim fp32 tensor (clip coefficient).
     Writes the refreshed low-precision shard into lowp_out (may be None)."""
-    g = grad.float()
+    g = grad.to(master.dtype) if master.dtype == torch.float64 else _f32(grad)
     if grad_scale is not None:
         g = g * grad_scale
     master.mul_(1.0 - lr * weight_decay)
