@@ -16,23 +16,20 @@
 // all-gather), warpgroups 1-2 = consumers (wgmma + epilogue).
 //
 // gemm_wide_bf16 is the same pipeline on a 128 x 256 tile (wgmma m64n256k16) for the GEMMs without fused communication;
-// use_wide picks the tile per launch.
+// use_wide picks the tile per launch.  Wherever TMA can describe its operands, the 128 x 256 tile runs with an epilogue
+// staged in shared memory instead (csrc/gemm_wide_sm90.cu); gemm_wide_bf16 serves the other operands and is the
+// bitwise reference.
 //
 // The operands of the fused epilogues (RoPE table and bias, SwiGLU aux, push table) come with each launch in a
 // GemmEpilogueArgs (gemm_epilogue.h); check_epilogue validates them for all three launch entries.
 #include "common.cuh"
 #include "gemm_epilogue.h"
+#include "gemm_sm90.cuh"
 #include "tensormap.h"
 #include "wgmma.cuh"
 
 namespace b200 {
 
-constexpr int BM = 128, BN = 128, BK = 64;   // BK in bf16 elements = one 128-byte swizzle atom per row
-constexpr int STAGES = 6;
-constexpr int A_BYTES = BM * BK * 2;          // 16 KiB
-constexpr int B_BYTES = BN * BK * 2;          // 16 KiB
-constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-constexpr int THREADS = 384;
 // push epilogue (bulk mode): each consumer warpgroup stages its 64 x 128 bf16 tile rows (row pitch 272 B: the 16-byte
 // pad spreads the rows of a warp's fragment stores over the banks) so every 64-column row chunk leaves the SM as ONE
 // 128-byte cp.async.bulk store; the ring gives up one stage to make room
@@ -43,31 +40,6 @@ __host__ __device__ constexpr int ring_stages() { return EPI == 4 /*EPI_PUSH*/ ?
 template <int EPI>
 __host__ __device__ constexpr int smem_bytes() {   // ring + 1 KiB alignment slack + barriers (+ push staging)
   return ring_stages<EPI>() * STAGE_BYTES + 1024 + 256 + (EPI == 4 ? PUSH_STAGE_BYTES : 0);
-}
-
-enum { EPI_STORE = 0, EPI_RESIDUAL = 1, EPI_ACCUM = 2, EPI_ROPE = 3, EPI_PUSH = 4, EPI_SWIGLU = 5, EPI_SWIGLU_BWD = 6,
-       EPI_SCALE = 7, EPI_ROPE_BIAS = 8 };
-// Grouped (mixture-of-experts) launches of the 128 x 128 kernel carry their mode in the high bits of the EPI template
-// argument, so the instantiations that existed before them keep their names and their code.  Operands live in the
-// expert-sorted row buffer of csrc/moe.cu; the expert weights are one tensor whose rows hold all experts.
-//   GRP_M (forward nt, dgrad nn): m-tile mt belongs to expert p.grp_tile[mt] (-1: past the last segment, the tile is
-//          skipped by producer and consumers alike); B's row (nt) or k (nn) coordinate is offset by e * p.grp_rows.
-//   GRP_K (wgrad tn): problem b0 = expert e of p.nb0; its k-loop covers the rows [start, start + len) of the buffer
-//          (p.grp_seg[e], p.grp_seg[nb0 + e]), rounded out to 64-row blocks that only add padding rows, which are zero;
-//          C of expert e starts at e * p.sc0.
-constexpr int EPI_MASK = 15, GRP_M = 16, GRP_K = 32;
-
-// L2-friendly rasterisation: sweep all n-tiles for a band of GROUP_M m-tiles before moving to the next band, so the
-// band's A rows stay L2-resident while B streams through once per band.
-constexpr int GROUP_M = 16;
-B200_DEVINL void tile_coords(int t, int m_tiles, int n_tiles, int& mt, int& nt) {
-  const int per_band = GROUP_M * n_tiles;
-  const int band = t / per_band;
-  const int first_m = band * GROUP_M;
-  const int band_m = min(GROUP_M, m_tiles - first_m);
-  const int r = t - band * per_band;
-  mt = first_m + r % band_m;
-  nt = r / band_m;
 }
 
 // ---- fused all-gather (ag_gemm): the comm warps of the same persistent GEMM pull a unit's parameter shards from the
@@ -123,49 +95,6 @@ B200_DEVINL void ag_wait_chunks(const AgParams& ag, unsigned long long byte_lo, 
   asm volatile("fence.proxy.async;" ::: "memory");  // generic-proxy writes of the comm warps -> TMA (async proxy) reads
 }
 
-struct GemmParams {
-  int M, N, K;          // C is [M,N], reduction length K
-  int ldc, ldr;         // row strides (elements) of C and residual
-  void* C;
-  const void* R;        // residual (bf16) or nullptr
-  int m_tiles, n_tiles;
-  // batched mode (BATCH = true): nb0 x nb1 independent problems; operands come through rank-4 tensor maps
-  // {inner, outer, b0, b1}; C of problem (b0, b1) starts at b0 * sc0 + b1 * sc1 elements
-  int nb0, nb1;
-  long long sc0, sc1;
-  // EPI_ROPE (QKV projection): rotate adjacent column pairs of the first rope_cols columns by the angle of
-  // (row % rope_S, (col % rope_hd) / 2) before the bf16 store; table is [S][hd/2][cos, sin] fp32 (SURVEY.md K2)
-  // Grouped launches never rotate, so they keep the expert tables in the same slots: grp_tile = the plan's tile table,
-  // grp_rows = weight rows per expert.
-  union { const float* rope; const int* grp_tile; };
-  union { int rope_S; int grp_rows; };
-  int rope_hd, rope_cols;
-  // EPI_PUSH (fused wgrad GEMM -> reduce-scatter, SURVEY.md N8): the wgrad tile is not stored to C but pushed over
-  // NVLink into the staging buffer of the rank that OWNS that slice of the unit's flat gradient:
-  //   e = push_off + row * ldc + col ; owner = e / push_n ; dst = push_bases[owner] + push_rank * push_n + (e - owner * push_n)
-  void* const* push_bases;
-  long long push_n, push_off;
-  int push_rank;
-  int push_bulk;        // 1: stage rows in shared memory, 128-byte bulk stores; 0: 4-byte stores from registers
-  // every CTA starts its sweep `tile_rot` tiles into the raster (wraps around).  The push epilogue sets it to
-  // rank * tiles / world so that the ranks, which run the same wgrad GEMM at the same time, write into different owners.
-  int tile_rot;
-  // EPI_SWIGLU (gate/up projection, nt): B is the fused [2F, K] weight.  A tile covers 64 features: accumulator columns
-  // [0,64) come from rows [f0, f0+64) of the FIRST half of the weight and [64,128) from the same features of the SECOND
-  // half, so every thread holds gate and up of the same feature: it stores the bf16 projection to C [M, 2F] (needed by
-  // the backward) AND silu(gate) * up to aux [M, F].  N of the launch = F.
-  // EPI_SWIGLU_BWD (down-projection dgrad, nn): the accumulator is dS [M, F]; the epilogue reads gate / up from
-  // aux = the saved projection [M, 2F] and stores d(gate) | d(up) to C [M, 2F] -- dS itself never reaches memory.
-  void* aux;
-  int ld_aux, swi_F, swi_gate_first;
-  // EPI_SCALE (fp8 e4m3 operands, FP8 = true): C = acc * scale_a[row] * scale_b[col].  GRP_K: grp_seg = the plan's
-  // [start | len] of every expert.
-  // EPI_ROPE_BIAS (QKV projection with q / k / v biases): bias [N] bf16 is added to the accumulator, then the q / k
-  // columns are rotated as in EPI_ROPE.  fp8 launches never rotate, so the bias shares scale_b's slot.
-  union { const float* scale_a; const int* grp_seg; };
-  union { const float* scale_b; const __nv_bfloat16* bias; };
-};
-
 B200_DEVINL void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
   asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;"
                ::"l"(gdst), "r"(smem_u32(ssrc)), "r"(bytes) : "memory");
@@ -175,19 +104,6 @@ B200_DEVINL void bulk_store_s2g(void* gdst, const void* ssrc, uint32_t bytes) {
 B200_DEVINL __nv_bfloat16* push_dst(const GemmParams& p, long long e) {
   const long long owner = e / p.push_n;
   return reinterpret_cast<__nv_bfloat16*>(p.push_bases[owner]) + ((long long)p.push_rank * p.push_n + (e - owner * p.push_n));
-}
-
-B200_DEVINL float sigmoidf_fast(float x) { return __frcp_rn(1.f + exp2f(-1.4426950408889634f * x)); }
-
-template <typename OutT>
-B200_DEVINL void store2(OutT* p, float a, float b) {
-  if constexpr (sizeof(OutT) == 2) *reinterpret_cast<uint32_t*>(p) = pack_bf16x2(a, b);
-  else *reinterpret_cast<float2*>(p) = make_float2(a, b);
-}
-template <typename OutT>
-B200_DEVINL float2 load2(const OutT* p) {
-  if constexpr (sizeof(OutT) == 2) return unpack_bf16x2(*reinterpret_cast<const uint32_t*>(p));
-  else return *reinterpret_cast<const float2*>(p);
 }
 
 // Epilogue of one column pair (col, col + 1) of one row; col is even and N is a multiple of 8.
@@ -542,15 +458,7 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
 // setmaxnreg hands the producer warpgroup's registers to the consumers (128 x 40 + 256 x 232 <= 64K).
 // Epilogues: store, +residual, accumulate (bf16 or fp32 output), RoPE (with or without bias), SwiGLU forward
 // (F % 128 == 0) and backward.
-constexpr int WBN = 256;
-constexpr int W_STAGES = 4;
-constexpr int W_STAGE_BYTES = A_BYTES + WBN * BK * 2;   // 16 + 32 KiB
 constexpr int W_SMEM_BYTES = W_STAGES * W_STAGE_BYTES + 1024 + 256;
-
-template <int N>
-B200_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N>
-B200_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 template <bool A_MN, bool B_MN, int EPI, typename OutT>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -668,8 +576,9 @@ static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   return (int)cudaGetLastError();
 }
 
-// 0: the launcher picks the tile; 1: always 128 x 128; 2: 128 x 256 wherever the epilogue allows it.  Set only by the
-// GEMM benchmark and the tests, which compare the two tiles on the same operands.
+// 0: the launcher picks the tile; 1: always 128 x 128; 2: 128 x 256 wherever the epilogue allows it; 3: as 2, with the
+// register epilogue (gemm_wide_bf16) instead of the staged one.  Set only by the GEMM benchmark and the tests, which
+// compare the tiles and epilogues on the same operands.
 static int g_tile_override = 0;
 
 // The wide tile moves less data per FLOP but halves the tile count, so it wins unless it leaves a worse last wave:
@@ -678,7 +587,7 @@ static int g_tile_override = 0;
 constexpr int WIDE_TILE_COST = 15;
 static bool use_wide(const GemmParams& p, int epi) {
   if (g_tile_override == 1 || (epi == EPI_SWIGLU && p.swi_F % 128)) return false;
-  if (g_tile_override == 2) return true;
+  if (g_tile_override >= 2) return true;
   const long long sm = sm_count();
   const long long n_wide = (epi == EPI_SWIGLU) ? p.swi_F / 128 : (p.N + WBN - 1) / WBN;
   const long long waves_narrow = ((long long)p.m_tiles * p.n_tiles + sm - 1) / sm;
@@ -686,10 +595,16 @@ static bool use_wide(const GemmParams& p, int epi) {
   return 2 * WIDE_TILE_COST * waves_wide <= 16 * waves_narrow;
 }
 
-// every GEMM of the single-GPU path (no fused all-gather, no push): one launch of the tile use_wide picks
+// every GEMM of the single-GPU path (no fused all-gather, no push): one launch of the tile use_wide picks.  The
+// 128 x 256 tile runs with the staged epilogue (csrc/gemm_wide_sm90.cu) wherever TMA can describe its operands.
 template <bool A_MN, bool B_MN, int EPI, typename OutT>
 static int launch_local(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
-  if (use_wide(p, EPI)) return launch_wide<A_MN, B_MN, EPI, OutT>(tmA, tmB, p, stream);
+  if (use_wide(p, EPI)) {
+    constexpr int fp32 = sizeof(OutT) == 4;
+    if (g_tile_override != 3 && b200_gemm_wide_staged_ok(&p, EPI, fp32))
+      return b200_gemm_wide_staged(&tmA, &tmB, &p, A_MN, B_MN, EPI, fp32, stream);
+    return launch_wide<A_MN, B_MN, EPI, OutT>(tmA, tmB, p, stream);
+  }
   return launch<A_MN, B_MN, EPI, OutT, false>(tmA, tmB, p, AgParams{}, stream);
 }
 
@@ -782,7 +697,7 @@ static int check_epilogue(const GemmEpilogueArgs& e, int epi, int N, int ldc, in
 }  // namespace b200
 
 // tile of the single-GPU GEMMs: 0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256 where the epilogue allows it
-extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode == 1 || mode == 2) ? mode : 0; }
+extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode >= 1 && mode <= 3) ? mode : 0; }
 
 // C[M,N] = op(A) op(B) (+R | +C | fused epilogue).  a_mn: A is stored [K,M] (M contiguous) else [M,K];  b_mn: B is
 // stored [K,N] (N contiguous) else [N,K].  lda/ldb/ldc/ldr are row strides in elements.  Returns 0 or an error code.

@@ -1,0 +1,221 @@
+"""The shared-memory epilogue of the 128 x 256 GEMM tile (``gemm_wide_bf16`` in csrc/gemm_sm90.cu): results leave through
+TMA stores and the epilogue operands arrive by TMA loads.  Every GEMM of the headline step at its real epilogue and
+output dtype, and the edges of the TMA boxes, must give the same bits as the 128 x 128 tile on the same operands, stay
+within the oracle's tolerance, and leave every element around C and aux untouched (the stores clip at M and N)."""
+import os
+import re
+import shutil
+import subprocess
+
+import pytest
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+DEV = "cuda"
+T, D, F, H, KVH, HD, V, S = 8192, 2048, 6144, 16, 4, 128, 32000, 4096
+QKV = (H + 2 * KVH) * HD
+LAYOUT = {"nt": 0, "nn": 1, "tn": 2}
+EPI = {"store": 0, "residual": 1, "accumulate": 2, "rope": 3, "swiglu": 5, "swiglu_bwd": 6, "rope_bias": 8}
+GUARD = 1234.0   # exact in bf16 and fp32
+
+# (name, layout, M, N, K, epilogue, output dtype, options); the SwiGLU forward's N is 2F, the rows of the fused weight.
+# options: ldc / ldr / ld_aux pads (elements past the row), gate_first, rope (hd, H, KVH, S), broadcast (residual)
+HEADLINE = [
+    ("qkv_fwd", "nt", T, QKV, D, "rope", torch.bfloat16, {}),
+    ("o_fwd", "nt", T, D, H * HD, "residual", torch.bfloat16, {}),
+    ("gateup_fwd", "nt", T, 2 * F, D, "swiglu", torch.bfloat16, {}),
+    ("down_fwd", "nt", T, D, F, "residual", torch.bfloat16, {}),
+    ("down_dgrad", "nn", T, F, D, "swiglu_bwd", torch.bfloat16, {}),
+    ("down_wgrad", "tn", D, F, T, "store", torch.bfloat16, {}),
+    ("gateup_dgrad", "nn", T, D, 2 * F, "store", torch.bfloat16, {}),
+    ("gateup_wgrad", "tn", 2 * F, D, T, "store", torch.bfloat16, {}),
+    ("o_dgrad", "nn", T, H * HD, D, "store", torch.bfloat16, {}),
+    ("o_wgrad", "tn", D, H * HD, T, "store", torch.bfloat16, {}),
+    ("qkv_dgrad", "nn", T, D, QKV, "store", torch.bfloat16, {}),
+    ("qkv_wgrad", "tn", QKV, D, T, "store", torch.bfloat16, {}),
+    ("head_logits", "nt", 4096, V, D, "store", torch.bfloat16, {}),
+    ("head_dh", "nn", 4096, D, V, "store", torch.bfloat16, {}),
+    ("head_dw", "tn", V, D, 4096, "accumulate", torch.bfloat16, {}),
+]
+EDGES = [
+    ("store_m1000", "nt", 1000, 512, 256, "store", torch.bfloat16, {}),
+    ("store_n520", "nn", 512, 520, 256, "store", torch.bfloat16, {}),
+    ("store_n776_ldc", "tn", 1000, 776, 192, "store", torch.bfloat16, {"ldc": 40}),
+    ("residual_ldr_ne_ldc", "nt", 1000, 776, 264, "residual", torch.bfloat16, {"ldc": 8, "ldr": 24}),
+    ("accum_ragged_ldc", "tn", 1000, 520, 200, "accumulate", torch.bfloat16, {"ldc": 16}),
+    ("fp32_store", "nn", 640, 1288, 256, "store", torch.float32, {"ldc": 8}),
+    ("fp32_accum", "tn", 1000, 520, 200, "accumulate", torch.float32, {"ldc": 4 * 8}),
+    # rope_cols = (H + KVH) * hd = 360 ends 8 columns into a 32-column subtile; positions wrap at S = 300
+    ("rope_cols_mid_subtile", "nt", 1000, (4 + 2 * 1) * 72, 256, "rope", torch.bfloat16, {"rope": (72, 4, 1, 300)}),
+    ("rope_bias_qwen_n1152", "nt", 1000, 1152, 896, "rope_bias", torch.bfloat16, {"rope": (64, 14, 2, 512)}),
+    ("rope_bias_qwen_n4608", "nt", 2048, 4608, 512, "rope_bias", torch.bfloat16, {"rope": (128, 28, 4, 1024)}),
+    ("swiglu_gate_first", "nt", 1000, 2 * 384, 256, "swiglu", torch.bfloat16, {"ldc": 8, "ld_aux": 16}),
+    ("swiglu_up_first", "nt", 512, 2 * 256, 256, "swiglu", torch.bfloat16, {"gate_first": False}),
+    ("swiglu_bwd_gate_first", "nn", 1000, 328, 256, "swiglu_bwd", torch.bfloat16, {"ldc": 8, "ld_aux": 24}),
+    ("swiglu_bwd_up_first", "nn", 512, 320, 256, "swiglu_bwd", torch.bfloat16, {"gate_first": False}),
+]
+# operands a TMA map cannot describe: the 128 x 256 tile keeps its register epilogue
+FALLBACK = [
+    ("fp32_residual", "nt", 1000, 776, 264, "residual", torch.float32, {}),
+    # row stride 0: the bias of the unfused QKV path rides in the residual epilogue as a broadcast row
+    ("broadcast_residual", "nt", 1000, 776, 264, "residual", torch.bfloat16, {"broadcast": True}),
+]
+
+
+@pytest.fixture(scope="module")
+def K():
+    from fms_fsdp_b200.ops import cuda_kernels as CK
+    from fms_fsdp_b200.ops import torch_kernels as TK
+    assert CK._C.__file__.endswith("_C.so")
+    return CK, TK
+
+
+def guarded(rows, cols, pad, dtype):
+    """A [rows, cols] view with row stride cols + pad into a buffer of GUARD values with 16 guard rows on each side."""
+    buf = torch.full((rows + 32, cols + pad), GUARD, dtype=dtype, device=DEV)
+    return buf, buf[16:16 + rows, :cols]
+
+
+def untouched(buf, rows, cols):
+    mask = torch.ones_like(buf, dtype=torch.bool)
+    mask[16:16 + rows, :cols] = False
+    return bool((buf[mask] == GUARD).all())
+
+
+def tile_rel(out, ref, bm=128, bn=256):
+    """Largest per-tile relative error: max |out - ref| / max |ref| over each bm x bn block."""
+    out, ref = out.float(), ref.float()
+    M, N = ref.shape
+    pm, pn = (-M) % bm, (-N) % bn
+    e = torch.nn.functional.pad((out - ref).abs(), (0, pn, 0, pm))
+    r = torch.nn.functional.pad(ref.abs(), (0, pn, 0, pm))
+    blk = lambda x: x.view((M + pm) // bm, bm, (N + pn) // bn, bn).amax(dim=(1, 3))
+    return (blk(e) / blk(r).clamp(min=1e-6)).max().item()
+
+
+def make_case(CK, TK, case):
+    """(run: () -> [(buffer, view)] of the outputs, fp32 oracle of each output)."""
+    name, layout, M, N, Kd, epi, odt, opt = case
+    g = torch.Generator(device=DEV).manual_seed(sum(map(ord, name)))
+    rnd = lambda *s, scale=1.0: (torch.randn(*s, generator=g, device=DEV) * scale).bfloat16()
+    gate_first = opt.get("gate_first", True)
+    if epi == "swiglu":
+        Fh = N // 2
+        x, w = rnd(M, Kd, scale=0.5), rnd(N, Kd, scale=Kd ** -0.5)
+
+        def run():
+            gu = guarded(M, N, opt.get("ldc", 0), torch.bfloat16)
+            act = guarded(M, Fh, opt.get("ld_aux", 0), torch.bfloat16)
+            CK._C.gemm(x, w, gu[1], 0, EPI[epi], None, aux=act[1], swiglu_F=Fh, gate_first=gate_first)
+            return [gu, act]
+        return run, [x.float() @ w.float().t(), None]
+    if epi == "swiglu_bwd":
+        dy, w2 = rnd(M, Kd, scale=0.5), rnd(Kd, N, scale=Kd ** -0.5)
+        gu_buf, gu = guarded(M, 2 * N, opt.get("ld_aux", 0), torch.bfloat16)
+        gu.copy_(rnd(M, 2 * N))
+
+        def run():
+            dgu = guarded(M, 2 * N, opt.get("ldc", 0), torch.bfloat16)
+            CK._C.gemm(dy, w2, dgu[1], 1, EPI[epi], None, aux=gu, swiglu_F=N, gate_first=gate_first)
+            return [dgu]
+        return run, [TK.swiglu_bwd(dy.float() @ w2.float(), gu.float(), gate_first)]
+    a = rnd(*((M, Kd) if layout != "tn" else (Kd, M)), scale=0.5)
+    b = rnd(*((N, Kd) if layout == "nt" else (Kd, N)), scale=Kd ** -0.5)
+    kw, r, ref = {}, None, TK.gemm(a.float(), b.float(), layout)
+    if epi in ("rope", "rope_bias"):
+        hd, h, kvh, Sr = opt.get("rope", (HD, H, KVH, S))
+        ang = torch.arange(Sr, device=DEV, dtype=torch.float32)[:, None] * (1e4 ** (-torch.arange(0, hd, 2, device=DEV) / hd))
+        table = torch.stack((ang.cos(), ang.sin()), -1).contiguous()
+        bias = rnd(N) if epi == "rope_bias" else None
+        kw = dict(rope_table=table, rope_S=Sr, rope_hd=hd, rope_cols=(h + kvh) * hd)
+        if bias is not None:
+            kw["bias"] = bias
+        ref = TK.gemm(a.float(), b.float(), layout, rope=(table, Sr, hd, h, kvh),
+                      bias=None if bias is None else bias.float())
+    if epi == "residual":
+        if opt.get("broadcast"):
+            r = rnd(1, N).expand(M, N)
+        else:
+            r = guarded(M, N, opt.get("ldr", 0), torch.bfloat16)[1]
+            r.copy_(rnd(M, N))
+        ref = ref + r.float()
+    c0 = rnd(M, N).to(odt) if epi == "accumulate" else None
+    if c0 is not None:
+        ref = ref + c0.float()
+
+    def run():
+        c = guarded(M, N, opt.get("ldc", 0), odt)
+        if c0 is not None:
+            c[1].copy_(c0)
+        CK._C.gemm(a, b, c[1], LAYOUT[layout], EPI[epi], r, **kw)
+        return [c]
+    return run, [ref]
+
+
+def check(K, case):
+    """Staged epilogue (tile mode 2), the register epilogue of the same tile (3) and the 128 x 128 tile (1): the same
+    bits, every element outside the outputs untouched, and within the oracle's tolerance."""
+    CK, TK = K
+    run, refs = make_case(CK, TK, case)
+    outs = {}
+    for mode in (2, 3, 1):
+        CK._C._set_gemm_tile(mode)
+        try:
+            n0 = CK.launch_count()
+            outs[mode] = run()
+            torch.cuda.synchronize()
+            assert CK.launch_count() == n0 + 1, "one launch of our kernel per GEMM"
+        finally:
+            CK._C._set_gemm_tile(0)
+    if case[5] == "swiglu":   # the activation of the bf16-rounded projection, as both kernels compute it
+        refs[1] = TK.swiglu_fwd(outs[1][0][1].float(), case[7].get("gate_first", True))
+    for (sb, sv), (rb, _), (nb, nv), ref in zip(outs[2], outs[3], outs[1], refs):
+        assert untouched(sb, *sv.shape), (case[0], "the staged epilogue wrote outside its output")
+        assert torch.equal(sb, nb), (case[0], "staged and 128 x 128 differ", (sv.float() - nv.float()).abs().max().item())
+        assert torch.equal(rb, nb), (case[0], "register epilogue and 128 x 128 differ")
+        assert tile_rel(sv, ref) < 1e-2, case[0]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", HEADLINE, ids=[c[0] for c in HEADLINE])
+def test_wide_epilogue_headline_shapes(K, case):
+    check(K, case)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", EDGES, ids=[c[0] for c in EDGES])
+def test_wide_epilogue_edges(K, case):
+    check(K, case)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("case", FALLBACK, ids=[c[0] for c in FALLBACK])
+def test_operands_tma_cannot_describe_run_the_register_epilogue(K, case):
+    check(K, case)
+
+
+def test_wide_epilogue_sass():
+    """Every output of the staged-epilogue instantiations leaves through TMA stores: no STG at all, no local memory."""
+    so = os.path.join(ROOT, "fms_fsdp_b200", "_gemm_wide.so")
+    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(so) or not os.path.exists(exe):
+        pytest.skip("needs the built extension and cuobjdump")
+    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
+    per, name = {}, None
+    for line in out.splitlines():
+        m = re.search(r"Function : (\S+)", line)
+        if m:
+            name = m.group(1) if "gemm_wide_staged_bf16" in m.group(1) else None
+            if name:
+                per[name] = []
+        elif name and "/*" in line:
+            per[name].append(line)
+    assert len(per) == 24, sorted(per)   # 4 layouts x (store, accumulate) x (bf16, fp32), +residual x 4, RoPE x 2, SwiGLU x 2
+    for k, lines in per.items():
+        body = "\n".join(lines)
+        assert re.search(r"HGMMA\.64x256x16\.F32\.BF16", body), k
+        assert re.search(r"UTMALDG\.2D", body), k
+        assert re.search(r"UTMASTG", body), k
+        assert not re.search(r"\bSTG\b", body), k
+        assert not re.search(r"\b(LDL|STL)\b", body), k
+
