@@ -111,3 +111,5 @@ class train_config:
     qk_norm: bool = False                    # Llama: per-head RMSNorm of q and k before RoPE (Qwen3 QK-norm), for any variant
     grad_accum_steps: int = 1                # micro-batches per optimizer step (global batch = world x batch_size x this)
     moe_aux_loss_coef: Optional[float] = None  # MoE Llama: load-balancing loss coefficient (None = the variant's value)
+    z_loss_coef: float = 0.0                 # output z-loss c: CE + c * mean lse(logits)^2 (PaLM / OLMo 2: 1e-5); 0 = off
+    moe_router_z_loss_coef: float = 0.0      # MoE Llama: ST-MoE router z-loss coefficient, mean over layers; 0 = off

@@ -98,6 +98,13 @@ DECL int b200_moe_combine_bwd(const void*, const void*, const float*, const int*
                               int, int, void*, float*, cudaStream_t);
 DECL int b200_moe_route_bwd(const float*, const int*, const float*, const float*, const int*, int, int, int, int, float,
                             void*, cudaStream_t);
+// z-loss kernels (csrc/losses_sm90.cu, fms_fsdp_b200/_losses.so)
+DECL int b200_ce_zloss_grad_inplace(void*, const long long*, const float*, float*, int, int, int, long long, float,
+                                    cudaStream_t);
+DECL int b200_loss_partials_reduce(const float*, int, int, const float*, float, float*, cudaStream_t);
+DECL int b200_router_z_parts(int);
+DECL int b200_router_z_fwd(const float*, int, int, float*, float*, cudaStream_t);
+DECL int b200_router_z_bwd(void*, const float*, const float*, int, int, float, cudaStream_t);
 DECL int b200_causal_conv1d_fwd(const void*, const void*, const void*, void*, int, int, int, int, int, cudaStream_t);
 DECL int b200_causal_conv1d_bwd(const void*, const void*, const void*, const void*, void*, float*, float*, int, int,
                                 int, int, int, cudaStream_t);
@@ -452,6 +459,65 @@ void ce_grad_inplace(at::Tensor& logits, const at::Tensor& labels, const at::Ten
   check(b200_ce_grad_inplace(logits.data_ptr(), (const long long*)labels.data_ptr(), n_valid.data_ptr<float>(),
                              loss_sum.data_ptr<float>(), logits.size(0), logits.size(1), logits.stride(0), ignore,
                              cur_stream()), "ce_grad_inplace");
+}
+// ---- z-loss (csrc/losses_sm90.cu)
+// In place on a logits chunk [rows, V]: logits -> [(1 + 2 z_coef lse) softmax - onehot] / n_valid; part [rows, 2] fp32
+// gets (CE, lse^2) of every row, 0 on ignored rows.
+void ce_zloss_grad_inplace(at::Tensor& logits, const at::Tensor& labels, const at::Tensor& n_valid, at::Tensor& part,
+                           int64_t ignore, double z_coef) {
+  c10::cuda::CUDAGuard guard(logits.device());
+  need(logits, "logits", at::kBFloat16);
+  need(labels, "labels", at::kLong);
+  need(n_valid, "n_valid", at::kFloat);
+  need(part, "part", at::kFloat);
+  TORCH_CHECK(logits.dim() == 2 && logits.stride(1) == 1 && labels.is_contiguous() && labels.numel() == logits.size(0),
+              "ce_zloss_grad_inplace: logits [rows, V] with unit inner stride, labels [rows]");
+  TORCH_CHECK(part.is_contiguous() && part.dim() == 2 && part.size(0) == logits.size(0) && part.size(1) == 2,
+              "ce_zloss_grad_inplace: part must be a contiguous [rows, 2] fp32 tensor");
+  check(b200_ce_zloss_grad_inplace(logits.data_ptr(), (const long long*)labels.data_ptr(), n_valid.data_ptr<float>(),
+                                   part.data_ptr<float>(), logits.size(0), logits.size(1), logits.stride(0), ignore,
+                                   (float)z_coef, cur_stream()), "ce_zloss_grad_inplace");
+}
+// [nstat] fp32 = scale * column sums of part [n, nstat] / max(denom, 1), summed in a fixed order
+at::Tensor loss_partials_reduce(const at::Tensor& part, const c10::optional<at::Tensor>& denom, double scale) {
+  c10::cuda::CUDAGuard guard(part.device());
+  need(part, "part", at::kFloat);
+  TORCH_CHECK(part.is_contiguous() && part.dim() == 2, "loss_partials_reduce: part must be a contiguous [n, nstat] tensor");
+  const float* d = nullptr;
+  if (denom.has_value()) {
+    need(*denom, "denom", at::kFloat);
+    TORCH_CHECK(denom->numel() == 1, "loss_partials_reduce: denom must be a scalar");
+    d = denom->data_ptr<float>();
+  }
+  auto out = at::empty({part.size(1)}, part.options());
+  check(b200_loss_partials_reduce(part.data_ptr<float>(), part.size(0), part.size(1), d, (float)scale,
+                                  out.data_ptr<float>(), cur_stream()), "loss_partials_reduce");
+  return out;
+}
+// (lse [T] fp32, z = mean_t lse_t^2 fp32 scalar) of the router logits [T, E] fp32
+std::vector<at::Tensor> router_z_fwd(const at::Tensor& logits) {
+  c10::cuda::CUDAGuard guard(logits.device());
+  need(logits, "logits", at::kFloat);
+  TORCH_CHECK(logits.dim() == 2 && logits.is_contiguous(), "router_z_fwd: logits must be contiguous [T, E]");
+  const int T = logits.size(0), E = logits.size(1);
+  TORCH_CHECK(T > 0, "router_z_fwd: no tokens");
+  auto lse = at::empty({T}, logits.options());
+  auto part = at::empty({b200_router_z_parts(T), 1}, logits.options());
+  check(b200_router_z_fwd(logits.data_ptr<float>(), T, E, lse.data_ptr<float>(), part.data_ptr<float>(), cur_stream()),
+        "router_z_fwd");
+  auto z = loss_partials_reduce(part, c10::nullopt, 1.0 / T);
+  return {lse, z.squeeze(0)};
+}
+// dl [T, E] bf16 += scale * lse_t * probs_te (fp32 math, one rounding to bf16), in place
+void router_z_bwd(at::Tensor& dl, const at::Tensor& probs, const at::Tensor& lse, double scale) {
+  c10::cuda::CUDAGuard guard(dl.device());
+  need(dl, "dl", at::kBFloat16);
+  need(probs, "probs", at::kFloat);
+  need(lse, "lse", at::kFloat);
+  TORCH_CHECK(dl.dim() == 2 && dl.is_contiguous() && probs.is_contiguous() && lse.is_contiguous() &&
+              probs.sizes() == dl.sizes() && lse.numel() == dl.size(0), "router_z_bwd: dl, probs [T, E], lse [T]");
+  check(b200_router_z_bwd(dl.data_ptr(), probs.data_ptr<float>(), lse.data_ptr<float>(), dl.size(0), dl.size(1),
+                          (float)scale, cur_stream()), "router_z_bwd");
 }
 void adamw(at::Tensor& master, const at::Tensor& grad, at::Tensor& m, at::Tensor& v,
            const c10::optional<at::Tensor>& lowp, double lr, double b1, double b2, double eps, double wd, int64_t step,
@@ -1121,6 +1187,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("embedding_bwd", &embedding_bwd);
   m.def("count_valid", &count_valid);
   m.def("ce_grad_inplace", &ce_grad_inplace);
+  m.def("ce_zloss_grad_inplace", &ce_zloss_grad_inplace);
+  m.def("loss_partials_reduce", &loss_partials_reduce, py::arg("part"), py::arg("denom") = py::none(),
+        py::arg("scale") = 1.0);
+  m.def("router_z_fwd", &router_z_fwd);
+  m.def("router_z_bwd", &router_z_bwd);
   m.def("adamw", &adamw);
   m.def("sumsq", &sumsq);
   m.def("attn_fwd", &attn_fwd, py::arg("qkv"), py::arg("B"), py::arg("S"), py::arg("H"), py::arg("KVH"), py::arg("hd"),

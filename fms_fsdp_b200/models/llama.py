@@ -72,6 +72,13 @@ class LLaMAConfig:
     moe_hidden_dim: int = 0
     moe_norm_topk: bool = True
     moe_aux_loss_coef: float = 0.0
+    # extension (not an fms field): z-losses.  z_loss_coef c adds c * mean_t lse_t^2 to the objective, lse_t the
+    # logsumexp of token t's output logits (PaLM, OLMo 2 use 1e-5); moe_router_z_loss_coef c_r adds the ST-MoE router
+    # z-loss c_r * mean_layers mean_t (logsumexp_e router_logits_te)^2.  Both gradients are folded into the fused
+    # kernels' backward, and the returned loss stays the cross-entropy (``LLaMA.z_loss()`` /
+    # ``LLaMA.moe_router_z_loss()`` report the terms).  0 runs exactly the kernels of a model without them.
+    z_loss_coef: float = 0.0
+    moe_router_z_loss_coef: float = 0.0
 
     @property
     def hidden_dim(self) -> int:
@@ -220,6 +227,7 @@ class MoEFeedForward(nn.Module):
         self.w1 = nn.Parameter(torch.empty(E, 2 * F, D, device=device, dtype=dtype))
         self.w2 = nn.Parameter(torch.empty(E, D, F, device=device, dtype=dtype))
         self.last_aux = None          # the load-balancing statistic of the last forward (device scalar)
+        self.last_router_z = None     # mean_t lse_t^2 of the router logits of the last forward (with a router z-loss)
 
     def reset_parameters(self):
         for w in (self.gate.weight, self.w1, self.w2):
@@ -229,6 +237,12 @@ class MoEFeedForward(nn.Module):
         cfg = self.config
         # the loss is the mean over layers: each block's share of the coefficient (read here, so that the gradient and
         # LLaMA.moe_aux_loss() always use the same value)
+        if cfg.moe_router_z_loss_coef > 0:
+            y, self.last_aux, self.last_router_z = ops.moe_mlp(
+                h, self.gate.weight, self.w1, self.w2, cfg.moe_top_k, cfg.moe_norm_topk,
+                cfg.moe_aux_loss_coef / cfg.nlayers, residual=residual,
+                router_z_coef=cfg.moe_router_z_loss_coef / cfg.nlayers, return_router_z=True)
+            return y
         y, self.last_aux = ops.moe_mlp(h, self.gate.weight, self.w1, self.w2, cfg.moe_top_k, cfg.moe_norm_topk,
                                        cfg.moe_aux_loss_coef / cfg.nlayers, residual=residual)
         return y
@@ -311,6 +325,7 @@ class LLaMA(nn.Module):
                                        getattr(cfg, "rope_scaling", None))
         self.layers = nn.ModuleList([LLaMABlock(cfg, self.rot_emb, device, dtype) for _ in range(cfg.nlayers)])
         self.dec_norm = RMSNorm(cfg.emb_dim, cfg.norm_eps, device, dtype)
+        self.last_z = None            # mean lse^2 of the output logits of the last loss forward (with a z-loss)
 
     def get_config(self) -> LLaMAConfig:
         return self.config
@@ -321,6 +336,28 @@ class LLaMA(nn.Module):
         if self.config.moe_num_experts <= 0 or self.layers[0].moe.last_aux is None:
             return None
         return torch.stack([blk.moe.last_aux for blk in self.layers]).mean() * self.config.moe_aux_loss_coef
+
+    def z_loss(self):
+        """z_loss_coef * mean lse^2 of the output logits of the last loss forward, as a device scalar (its gradient is
+        already part of the backward); None without a z-loss or before the first forward with labels."""
+        if self.config.z_loss_coef <= 0 or self.last_z is None:
+            return None
+        return self.last_z * self.config.z_loss_coef
+
+    def moe_router_z_loss(self):
+        """moe_router_z_loss_coef * mean over layers of the router z statistic of the last forward, as a device scalar
+        (its gradient is already part of the backward); None without a router z-loss or before the first forward."""
+        cfg = self.config
+        if cfg.moe_num_experts <= 0 or cfg.moe_router_z_loss_coef <= 0 or self.layers[0].moe.last_router_z is None:
+            return None
+        return torch.stack([blk.moe.last_router_z for blk in self.layers]).mean() * cfg.moe_router_z_loss_coef
+
+    def _loss(self, h, labels, ignore_index=-100):
+        if self.config.z_loss_coef > 0:
+            ce, self.last_z = ops.linear_cross_entropy_z(h, self.shared.head.weight, labels, self.config.z_loss_coef,
+                                                         ignore_index)
+            return ce
+        return ops.linear_cross_entropy(h, self.shared.head.weight, labels, ignore_index)
 
     def reset_parameters(self):
         self.shared.reset_parameters()
@@ -346,7 +383,7 @@ class LLaMA(nn.Module):
         if return_hidden:
             return h
         if labels is not None:
-            return ops.linear_cross_entropy(h, self.shared.head.weight, labels)
+            return self._loss(h, labels)
         return self.shared(h, reverse=True)
 
     # ---- sharded-runtime protocol -------------------------------------------------------------
@@ -372,7 +409,7 @@ class LLaMA(nn.Module):
         h = self.dec_norm(h)
         if labels is None:
             return self.shared(h, reverse=True)
-        return ops.linear_cross_entropy(h, self.shared.head.weight, labels, ignore_index)
+        return self._loss(h, labels, ignore_index)
 
 
 def param_count(model: nn.Module) -> int:

@@ -386,6 +386,10 @@ class MambaLMHeadModel(nn.Module):
         self.lm_head = _W(config.padded_vocab, config.d_model, device, dtype)
         if config.tie_embeddings:
             self.lm_head.weight = self.backbone.embedding.weight
+        # output z-loss coefficient c (objective CE + c * mean_t lse_t^2, lse_t the logsumexp of token t's logits).  It
+        # lives on the model, not in MambaConfig, whose fields are those of mamba_ssm's config.
+        self.z_loss_coef = 0.0
+        self.last_z = None
 
     def reset_parameters(self):
         cfg = self.config
@@ -427,7 +431,18 @@ class MambaLMHeadModel(nn.Module):
         hidden, _ = ops.add_rmsnorm(hidden, residual, nf.weight, nf.eps, self.config.residual_in_fp32)
         if labels is None:
             return ops.linear(hidden, self.lm_head.weight)
+        if self.z_loss_coef > 0:
+            ce, self.last_z = ops.linear_cross_entropy_z(hidden, self.lm_head.weight, labels, self.z_loss_coef,
+                                                         ignore_index)
+            return ce
         return ops.linear_cross_entropy(hidden, self.lm_head.weight, labels, ignore_index)
+
+    def z_loss(self):
+        """z_loss_coef * mean lse^2 of the output logits of the last loss forward (device scalar; its gradient is
+        already part of the backward); None without a z-loss or before the first forward with labels."""
+        if self.z_loss_coef <= 0 or self.last_z is None:
+            return None
+        return self.last_z * self.z_loss_coef
 
     # ---- mamba_ssm-style export (config.json + pytorch_model.bin)
     def save_pretrained(self, save_directory):

@@ -579,6 +579,64 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100):
     return loss_sum / n_valid.clamp(min=1.0), g
 
 
+# ------------------------------------------------------------------- z-loss (csrc/losses_sm90.cu, _losses.so)
+def linear_ce_z_fwd_bwd(h, w, labels, dw_out, z_coef, ignore_index=-100, chunk_rows=4096, accumulate=False):
+    """(CE, z, dh): ``linear_ce_fwd_bwd`` with the output z-loss inside the gradient kernel.  Each row's CE and lse^2
+    go to a per-row partial; one CTA sums them in a fixed order (the same bits on every run)."""
+    M, D = h.shape
+    V = w.shape[0]
+    if h.dtype != torch.bfloat16 or V % 8 or D % 8 or M % 8:
+        return _fallback("linear_ce_z_fwd_bwd").linear_ce_z_fwd_bwd(h, w, labels, dw_out, z_coef, ignore_index,
+                                                                    chunk_rows, accumulate)
+    labels = labels.reshape(-1)
+    if labels.dtype != torch.long:
+        labels = labels.long()
+    n_valid = torch.zeros((), dtype=torch.float32, device=h.device)
+    _C.count_valid(labels, ignore_index, n_valid)
+    part = torch.empty(M, 2, dtype=torch.float32, device=h.device)
+    dh = torch.empty_like(h)
+    chunk_rows = min(chunk_rows, M)
+    logits = torch.empty(chunk_rows, V, dtype=torch.bfloat16, device=h.device)
+    first = not accumulate
+    for s in range(0, M, chunk_rows):
+        e = min(M, s + chunk_rows)
+        lg = logits[: e - s]
+        gemm(h[s:e], w, "nt", out=lg)
+        _C.ce_zloss_grad_inplace(lg, labels[s:e], n_valid, part[s:e], ignore_index, float(z_coef))
+        gemm(lg, w, "nn", out=dh[s:e])
+        gemm(lg, h[s:e], "tn", out=dw_out, accumulate=not first)
+        first = False
+    stats = _C.loss_partials_reduce(part, n_valid, 1.0)          # (CE, z), each over max(n_valid, 1)
+    return stats[0], stats[1], dh
+
+
+def cross_entropy_z_fwd_bwd(logits, labels, z_coef, ignore_index=-100):
+    V = logits.shape[-1]
+    if logits.dtype != torch.bfloat16 or V % 8:
+        return _fallback("cross_entropy_z_fwd_bwd").cross_entropy_z_fwd_bwd(logits, labels, z_coef, ignore_index)
+    labels = labels.reshape(-1).long()
+    n_valid = torch.zeros((), dtype=torch.float32, device=logits.device)
+    _C.count_valid(labels, ignore_index, n_valid)
+    g = logits.clone()
+    part = torch.empty(g.shape[0], 2, dtype=torch.float32, device=logits.device)
+    _C.ce_zloss_grad_inplace(g, labels, n_valid, part, ignore_index, float(z_coef))
+    stats = _C.loss_partials_reduce(part, n_valid, 1.0)
+    return stats[0], stats[1], g
+
+
+def router_z_fwd(logits):
+    """(lse [T] fp32, z = mean_t lse_t^2) of the fp32 router logits [T, E]."""
+    lse, z = _C.router_z_fwd(logits.float().contiguous())
+    return lse, z
+
+
+def router_z_bwd(dl, probs, lse, scale):
+    """In place on the router-logit gradient: dl += scale * lse_t * p_te.  ``moe_route_bwd`` hands the gradient over
+    in bf16, so the term is added in fp32 to the rounded value and rounded once more."""
+    _C.router_z_bwd(dl, probs, lse, float(scale))
+    return dl
+
+
 # ------------------------------------------------------------------------------------- optimizer
 def sumsq(x, out=None):
     if out is None:

@@ -512,11 +512,11 @@ def gated_mlp(x, wg1, w2, residual: Optional[torch.Tensor] = None, gate_first: b
 class _MoEMLP(torch.autograd.Function):
     """Dropless top-k mixture of SwiGLU experts as ONE node.  Forward: router GEMM (fp32 logits), route, plan, permute,
     the m-grouped gate/up GEMM with the SwiGLU epilogue, the m-grouped down GEMM, combine (+ residual).  Backward: the
-    mirror image, with the load-balancing loss's gradient added inside the routing backward.  Every step is
-    deterministic, so a recomputed forward routes exactly as the first one did."""
+    mirror image, with the load-balancing loss's gradient added inside the routing backward (and the router z-loss's
+    after it).  Every step is deterministic, so a recomputed forward routes exactly as the first one did."""
 
     @staticmethod
-    def forward(ctx, h, router_w, w1, w2, residual, top_k, norm_topk, aux_coef):
+    def forward(ctx, h, router_w, w1, w2, residual, top_k, norm_topk, aux_coef, z_coef, want_z):
         K = kernels_for(h)
         D = h.shape[-1]
         h2 = h.reshape(-1, D)
@@ -525,22 +525,28 @@ class _MoEMLP(torch.autograd.Function):
         E = wr.shape[0]
         logits = K.gemm(h2, wr, "nt", out_dtype=torch.float32)
         ids, wts, probs = K.moe_route(logits, top_k, norm_topk)
+        lse = z = None
+        if z_coef > 0 or want_z:
+            lse, z = K.router_z_fwd(logits)      # the backward has probs but not the logits: keep lse
         plan, aux = K.moe_plan(ids, probs)
         xp = K.moe_permute(h2, plan, top_k, E)
         hp, sp = K.moe_up_fwd(xp, _wdata(w1), plan, T, top_k)
         yp = K.moe_down_fwd(sp, _wdata(w2), plan, T, top_k)
         y = K.moe_combine(yp, plan, wts, None if residual is None else residual.reshape(-1, D), E)
         ctx.K, ctx.ws, ctx.has_res = K, (router_w, w1, w2), residual is not None
-        ctx.args = (T, E, top_k, norm_topk, aux_coef * E / (T * T))
-        ctx.save_for_backward(h, ids, wts, probs, plan, xp, hp, sp, yp)
-        ctx.mark_non_differentiable(aux)
-        return y.view(h.shape), aux
+        ctx.args = (T, E, top_k, norm_topk, aux_coef * E / (T * T), 2 * z_coef / T)
+        ctx.save_for_backward(h, ids, wts, probs, plan, xp, hp, sp, yp, lse if z_coef > 0 else None)
+        if not want_z:
+            ctx.mark_non_differentiable(aux)
+            return y.view(h.shape), aux
+        ctx.mark_non_differentiable(aux, z)
+        return y.view(h.shape), aux, z
 
     @staticmethod
-    def backward(ctx, dy, _daux):
-        h, ids, wts, probs, plan, xp, hp, sp, yp = ctx.saved_tensors
+    def backward(ctx, dy, _daux, _dz=None):
+        h, ids, wts, probs, plan, xp, hp, sp, yp, lse = ctx.saved_tensors
         K, (router_w, w1, w2) = ctx.K, ctx.ws
-        T, E, k, norm_topk, aux_scale = ctx.args
+        T, E, k, norm_topk, aux_scale, z_scale = ctx.args
         h2 = h.reshape(T, -1)
         dyp, dw = K.moe_combine_bwd(dy.reshape(T, -1), yp, plan, wts, E)
         dhp = K.moe_down_bwd(dyp, _wdata(w2), hp, plan, T, k)
@@ -550,24 +556,34 @@ class _MoEMLP(torch.autograd.Function):
         dw1 = _deliver_wgrad(w1, lambda out, acc: K.moe_wgrad(dhp, xp, plan, T, k, out, acc)) \
             if ctx.needs_input_grad[2] else None
         dh = K.moe_permute_bwd(dxp, plan, T, k, E)
-        dl = K.moe_route_bwd(probs, ids, wts, dw, plan, norm_topk, aux_scale).to(h.dtype)
+        dl = K.moe_route_bwd(probs, ids, wts, dw, plan, norm_topk, aux_scale)
+        if lse is not None:                      # router z-loss: d(z_coef mean_t lse_t^2) = 2 z_coef / T lse_t p_te
+            dl = K.router_z_bwd(dl, probs, lse, z_scale)
+        dl = dl.to(h.dtype)
         dh = K.gemm(dl, _wdata(router_w), "nn", residual=dh).view_as(h)
         dwr = _deliver_wgrad(router_w, lambda out, acc: K.gemm(dl, h2, "tn", out=out, accumulate=acc)) \
             if ctx.needs_input_grad[1] else None
-        return dh, dwr, dw1, dw2, (dy if ctx.has_res else None), None, None, None
+        return dh, dwr, dw1, dw2, (dy if ctx.has_res else None), None, None, None, None, None
 
 
-def moe_mlp(h, router_w, w1, w2, top_k, norm_topk=False, aux_coef=0.0, residual: Optional[torch.Tensor] = None):
+def moe_mlp(h, router_w, w1, w2, top_k, norm_topk=False, aux_coef=0.0, residual: Optional[torch.Tensor] = None,
+            router_z_coef=0.0, return_router_z=False):
     """Dropless top-k mixture of SwiGLU experts: ``residual + sum_s w_s * expert_{e_s}(h)`` per token.
 
     router_w [E, D]; w1 [E, 2F, D] (each expert's [gate | up], like ``wg1_fused``); w2 [E, D, F].  Routing: fp32 softmax
     of ``h @ router_w^T``, the ``top_k`` experts by logit (ties to the lower index), weights = their probabilities,
     renormalised to sum to 1 when ``norm_topk``.  Returns ``(y, aux)`` with aux = E * sum_e (count_e / T) * mean_t p_te,
     the Switch load-balancing statistic of this call (a detached fp32 scalar on the device).  Its gradient, scaled by
-    ``aux_coef``, is added to the router's in backward: callers do not add ``aux`` to their loss."""
+    ``aux_coef``, is added to the router's in backward: callers do not add ``aux`` to their loss.
+
+    Router z-loss (ST-MoE): z = mean_t (logsumexp_e router_logits_te)^2 of this call.  With ``router_z_coef`` > 0 the
+    gradient of ``router_z_coef * z`` is added to the router's in backward, like the load-balancing gradient.
+    ``return_router_z=True`` returns ``(y, aux, z)``, z a detached fp32 device scalar; with both left at their
+    defaults the call runs exactly the kernels it runs without a z-loss."""
     if _GEMM_PRECISION == "fp8":
         raise NotImplementedError("moe_mlp: the grouped expert GEMMs are bf16 only")
-    return _MoEMLP.apply(h, router_w, w1, w2, residual, int(top_k), bool(norm_topk), float(aux_coef))
+    return _MoEMLP.apply(h, router_w, w1, w2, residual, int(top_k), bool(norm_topk), float(aux_coef),
+                         float(router_z_coef), bool(return_router_z))
 
 
 class _AddRMSNorm(torch.autograd.Function):
@@ -640,28 +656,36 @@ def set_unit_upstream(flag: bool):
     _UNIT_UPSTREAM = bool(flag)
 
 
+def _linear_ce_forward(ctx, h, w, run):
+    """Forward of the fused head nodes: ``run(K, h2, w, dw_out, accumulate)`` returns (*statistics, dh) with dh and dW
+    for an upstream gradient of 1; returns the statistics."""
+    K = kernels_for(h)
+    h2 = h.reshape(-1, h.shape[-1])
+    buf = getattr(w, "_grad_buf", None)
+    ctx.buf = None
+    if buf is not None:
+        # the runtime bound the root unit's gradient buffer before the head: dW lands there directly (no [V, D]
+        # temporary, no copy in collect_grads)
+        acc = bool(getattr(w, "_grad_ready", False))
+        *stats, dh = run(K, h2, _wdata(w), buf, acc)
+        w._grad_ready = True
+        ctx.dw = None
+        ctx.buf, ctx.buf_accumulated = buf, acc
+    else:
+        dw = torch.zeros_like(_wdata(w))
+        *stats, dh = run(K, h2, _wdata(w), dw, False)
+        ctx.dw = dw
+    ctx.w = w
+    ctx.save_for_backward(dh)
+    ctx.shape = h.shape
+    return stats
+
+
 class _LinearCE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, h, w, labels, ignore_index):
-        K = kernels_for(h)
-        h2 = h.reshape(-1, h.shape[-1])
-        buf = getattr(w, "_grad_buf", None)
-        ctx.buf = None
-        if buf is not None:
-            # the runtime bound the root unit's gradient buffer before the head: dW lands there directly (no [V, D]
-            # temporary, no copy in collect_grads)
-            acc = bool(getattr(w, "_grad_ready", False))
-            loss, dh = K.linear_ce_fwd_bwd(h2, _wdata(w), labels, buf, ignore_index, accumulate=acc)
-            w._grad_ready = True
-            ctx.dw = None
-            ctx.buf, ctx.buf_accumulated = buf, acc
-        else:
-            dw = torch.zeros_like(_wdata(w))
-            loss, dh = K.linear_ce_fwd_bwd(h2, _wdata(w), labels, dw, ignore_index)
-            ctx.dw = dw
-        ctx.w = w
-        ctx.save_for_backward(dh)
-        ctx.shape = h.shape
+        (loss,) = _linear_ce_forward(ctx, h, w, lambda K, h2, wd, dw, acc: K.linear_ce_fwd_bwd(
+            h2, wd, labels, dw, ignore_index, accumulate=acc))
         return loss
 
     @staticmethod
@@ -686,6 +710,26 @@ def linear_cross_entropy(h, w, labels, ignore_index=-100):
     return _LinearCE.apply(h, w, labels, ignore_index)
 
 
+class _LinearCEZ(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, h, w, labels, ignore_index, z_coef):
+        ce, z = _linear_ce_forward(ctx, h, w, lambda K, h2, wd, dw, acc: K.linear_ce_z_fwd_bwd(
+            h2, wd, labels, dw, z_coef, ignore_index, accumulate=acc))
+        ctx.mark_non_differentiable(z)
+        return ce, z
+
+    @staticmethod
+    def backward(ctx, dloss, _dz):
+        return _LinearCE.backward(ctx, dloss) + (None,)
+
+
+def linear_cross_entropy_z(h, w, labels, z_loss_coef, ignore_index=-100):
+    """``linear_cross_entropy`` with the output z-loss (PaLM): returns ``(ce, z)``, ce the mean CE as there and
+    z = mean over the non-ignored rows of logsumexp(h @ w^T)^2, a detached fp32 device scalar.  The gradient is that of
+    ``ce + z_loss_coef * z``: it is folded into ce's, so callers do not add z to their loss."""
+    return _LinearCEZ.apply(h, w, labels, ignore_index, float(z_loss_coef))
+
+
 class _CE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, logits, labels, ignore_index):
@@ -703,6 +747,26 @@ class _CE(torch.autograd.Function):
 
 def cross_entropy(logits, labels, ignore_index=-100):
     return _CE.apply(logits, labels, ignore_index)
+
+
+class _CEZ(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, logits, labels, ignore_index, z_coef):
+        K = kernels_for(logits)
+        ce, z, dlogits = K.cross_entropy_z_fwd_bwd(logits.reshape(-1, logits.shape[-1]), labels, z_coef, ignore_index)
+        ctx.save_for_backward(dlogits)
+        ctx.shape = logits.shape
+        ctx.mark_non_differentiable(z)
+        return ce, z
+
+    @staticmethod
+    def backward(ctx, dloss, _dz):
+        return _CE.backward(ctx, dloss) + (None,)
+
+
+def cross_entropy_z(logits, labels, z_loss_coef, ignore_index=-100):
+    """``cross_entropy`` on materialised logits with the output z-loss: ``(ce, z)`` as ``linear_cross_entropy_z``."""
+    return _CEZ.apply(logits, labels, ignore_index, float(z_loss_coef))
 
 
 # ------------------------------------------------------------------------------------------- mamba

@@ -577,6 +577,65 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100):
 
 
 # ----------------------------------------------------------------------------------------------
+# z-loss (csrc/losses_sm90.cu).  Output z-loss: z = (1/n) sum over non-ignored rows of lse_t^2, lse_t the logsumexp of
+# row t's logits; the gradient returned is that of CE + c z, i.e. [(1 + 2 c lse_t) softmax - onehot] / n.  Router z-loss:
+# z = mean_t lse_t^2 of the router logits; its gradient scale * lse_t * p_te is added to the router-logit gradient.
+# ----------------------------------------------------------------------------------------------
+def _ce_z_grad(logits, lab, ok, n_valid, z_coef):
+    """(sum CE, sum lse^2, gradient of CE + c z) of a row block; logits already in the math dtype."""
+    lse = torch.logsumexp(logits, dim=-1)
+    safe = lab.clamp(min=0)
+    tgt = logits.gather(1, safe.unsqueeze(1)).squeeze(1)
+    p = torch.exp(logits - lse.unsqueeze(1)) * (1 + 2 * z_coef * lse).unsqueeze(1)
+    p.scatter_add_(1, safe.unsqueeze(1), -torch.ones_like(tgt).unsqueeze(1))
+    return ((lse - tgt) * ok).sum(), (lse * lse * ok).sum(), p * (ok.unsqueeze(1) / n_valid)
+
+
+def linear_ce_z_fwd_bwd(h, w, labels, dw_out, z_coef, ignore_index=-100, chunk_rows=4096, accumulate=False):
+    """``linear_ce_fwd_bwd`` with the output z-loss: returns (CE, z, dh); dW of CE + c z goes to ``dw_out``."""
+    M, D = h.shape
+    labels = labels.reshape(-1).long()
+    valid = labels != ignore_index
+    acc_t = _f32(h).dtype
+    n_valid = valid.sum().clamp(min=1).to(acc_t)
+    dh = torch.empty_like(h)
+    ce = torch.zeros((), dtype=acc_t, device=h.device)
+    z = torch.zeros((), dtype=acc_t, device=h.device)
+    first = not accumulate
+    for s in range(0, M, chunk_rows):
+        e = min(M, s + chunk_rows)
+        c_s, z_s, p = _ce_z_grad(_f32(h[s:e] @ w.t()), labels[s:e], valid[s:e], n_valid, z_coef)
+        ce, z = ce + c_s, z + z_s
+        p = p.to(h.dtype)
+        dh[s:e] = p @ w
+        gemm(p, h[s:e], "tn", out=dw_out, accumulate=not first)
+        first = False
+    return ce / n_valid, z / n_valid, dh
+
+
+def cross_entropy_z_fwd_bwd(logits, labels, z_coef, ignore_index=-100):
+    """``cross_entropy_fwd_bwd`` with the output z-loss: (CE, z, dlogits of CE + c z)."""
+    labels = labels.reshape(-1).long()
+    valid = labels != ignore_index
+    lf = _f32(logits)
+    n_valid = valid.sum().clamp(min=1).to(lf.dtype)
+    ce, z, p = _ce_z_grad(lf, labels, valid, n_valid, z_coef)
+    return ce / n_valid, z / n_valid, p.to(logits.dtype)
+
+
+def router_z_fwd(logits):
+    """(lse [T], z = mean_t lse_t^2) of the router logits [T, E]."""
+    lse = torch.logsumexp(_f32(logits), dim=-1)
+    return lse, (lse * lse).mean()
+
+
+def router_z_bwd(dl, probs, lse, scale):
+    """dl [T, E] += scale * lse_t * probs_te (in place; the gradient of scale / 2 * sum_t lse_t^2)."""
+    dl += (scale * _f32(lse).unsqueeze(1) * _f32(probs)).to(dl.dtype)
+    return dl
+
+
+# ----------------------------------------------------------------------------------------------
 # Optimizer / gradient utilities on flat shards
 # ----------------------------------------------------------------------------------------------
 def sumsq(x, out=None):

@@ -23,6 +23,7 @@ from functools import partial
 import torch
 import torch.distributed as dist
 
+from fms_fsdp_b200 import ops
 from fms_fsdp_b200.policies import (apply_fsdp_checkpointing, bfSixteen, fpSixteen, get_wrapper,
                                     param_init_function)
 
@@ -293,6 +294,11 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
     # MoE: the load-balancing loss of every micro-batch, summed on the device and read at report steps only
     inner = getattr(model, "module", model)
     moe_aux = torch.zeros((), device=device) if getattr(mcfg, "moe_num_experts", 0) > 0 else None
+    # z-losses (coefficient-scaled), summed the same way; reported only when their coefficient is set
+    z_coef = float(getattr(cfg, "z_loss_coef", 0.0) or 0.0)
+    z_sum = torch.zeros((), device=device) if z_coef > 0 else None
+    router_z_sum = torch.zeros((), device=device) if float(getattr(cfg, "moe_router_z_loss_coef", 0.0) or 0.0) > 0 \
+        else None
 
     ev0 = ev1 = None
     if is_cuda:
@@ -315,17 +321,27 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
             label = to_device(label)
             if engine_mode and cfg.fused_cross_entropy:
                 micro_loss = model.forward_backward(input, label.long() if label.dtype != torch.long else label)
+                if z_sum is not None:
+                    z_sum += inner.z_loss().to(z_sum.device)
             else:
                 output = model(input)
                 output = output.logits if hasattr(output, "logits") else output
-                micro_loss = torch.nn.functional.cross_entropy(output.view(-1, output.size(-1)).float(),
-                                                               label.view(-1).long())
+                if z_sum is not None:
+                    # the output z-loss on the materialised logits: its gradient is folded into micro_loss's
+                    micro_loss, micro_z = ops.cross_entropy_z(output.view(-1, output.size(-1)), label.view(-1).long(),
+                                                              z_coef)
+                    z_sum += micro_z.to(z_sum.device) * z_coef
+                else:
+                    micro_loss = torch.nn.functional.cross_entropy(output.view(-1, output.size(-1)).float(),
+                                                                   label.view(-1).long())
                 del output
                 micro_loss.backward()
                 micro_loss = micro_loss.detach()
             loss = micro_loss if loss is None else loss + micro_loss
             if moe_aux is not None:
                 moe_aux += inner.moe_aux_loss().to(moe_aux.device)
+            if router_z_sum is not None:
+                router_z_sum += inner.moe_router_z_loss().to(router_z_sum.device)
         if accum > 1:
             loss = loss / accum
         gnorm = model.clip_grad_norm_(cfg.grad_clip_thresh)
@@ -361,6 +377,9 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 dist.all_reduce(ddp_stats, op=dist.ReduceOp.SUM)
                 if moe_aux is not None:
                     dist.all_reduce(moe_aux, op=dist.ReduceOp.SUM)
+                for t_ in (z_sum, router_z_sum):
+                    if t_ is not None:
+                        dist.all_reduce(t_, op=dist.ReduceOp.SUM)
             train_loss = ddp_stats[0] / ddp_stats[2]
             g_norm = ddp_stats[1] / ddp_stats[2]
             # failure detection the reference lacks (SURVEY.md 5.3): a non-finite loss / grad norm is surfaced at the
@@ -391,6 +410,14 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                 print("gradient norm:", current_gnorm)
                 if moe_aux is not None:   # coef * mean over layers, micro-batches, steps and ranks
                     print("moe_aux_loss:", moe_aux.item() / (ddp_stats[2].item() * accum))
+                # coef * mean over micro-batches, steps and ranks (and layers for the router's)
+                z_report = {}
+                if z_sum is not None:
+                    z_report["z_loss"] = z_sum.item() / (ddp_stats[2].item() * accum)
+                if router_z_sum is not None:
+                    z_report["moe_router_z_loss"] = router_z_sum.item() / (ddp_stats[2].item() * accum)
+                for k_, v_ in z_report.items():
+                    print(f"{k_}:", v_)
                 print("reserved memory:", reserved_mem)
                 print("allocated memory:", allocated_mem)
                 print("current step time:", current_step_time)
@@ -415,13 +442,15 @@ def train(cfg, model, local_rank, rank, train_loader, optimizer, scheduler, prof
                         "overall throughput (token per gpu per sec)": overall_throughput,
                         "gpu reserved memory": reserved_mem,
                         "gpu allocated memory": allocated_mem,
+                        **z_report,
                     }, step=batch_idx)
             start = time.time()
             if is_cuda:
                 ev0.record()
             ddp_stats.zero_()
-            if moe_aux is not None:
-                moe_aux.zero_()
+            for t_ in (moe_aux, z_sum, router_z_sum):
+                if t_ is not None:
+                    t_.zero_()
         if is_cuda:
             torch.cuda.reset_peak_memory_stats(device)
 

@@ -69,6 +69,11 @@ def main(**kwargs):
                              "GEMMs are bf16 only")
         if cfg.moe_aux_loss_coef is not None:
             llama_config.moe_aux_loss_coef = float(cfg.moe_aux_loss_coef)
+        llama_config.moe_router_z_loss_coef = float(cfg.moe_router_z_loss_coef)
+    elif cfg.moe_router_z_loss_coef:
+        raise ValueError("--moe_router_z_loss_coef needs a mixture-of-experts variant: a dense model has no router")
+    if cfg.z_loss_coef:
+        llama_config.z_loss_coef = float(cfg.z_loss_coef)
     if cfg.low_cpu_fsdp or use_cuda:
         # one unit at a time is materialised directly on the device by the sharded runtime
         with torch.device("meta"):

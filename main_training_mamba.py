@@ -32,6 +32,9 @@ def main(**kwargs):
     if cfg.qk_norm:
         raise ValueError("--qk_norm is not supported for Mamba models: their attention layers have no q / k norm "
                          "weights, and the option would silently change nothing")
+    if cfg.moe_router_z_loss_coef:
+        raise ValueError("--moe_router_z_loss_coef is not supported for Mamba models: they have no mixture-of-experts "
+                         "router")
 
     use_cuda = torch.cuda.is_available() and cfg.comm_backend != "gloo"
     if use_cuda:
@@ -64,6 +67,7 @@ def main(**kwargs):
     else:
         model = MambaLMHeadModel(mamba_config)
         model.reset_parameters()
+    model.z_loss_coef = float(cfg.z_loss_coef)
 
     if rank == 0:
         total_params = sum(p.numel() for p in model.parameters() if p.requires_grad)
