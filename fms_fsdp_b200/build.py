@@ -6,12 +6,7 @@
 * every ``csrc/*.cu`` is torch-free and compiled by nvcc for ``compute_90a/sm_90a`` with ``-lineinfo``
   (ncu source pages) -- nvcc cross-compiles without a GPU;
 * ``csrc/bindings.cpp`` (torch/pybind) is compiled by g++ only;
-* the .so stays in the tree (git-ignored), next to the package, so the package imports from the source tree;
-* side libraries, each one ``.cu`` linked into a ``.so`` of its own that ``_C.so`` links (rpath ``$ORIGIN``), so that the
-  kernels of ``_C.so`` keep the instructions their recorded digests pin (``tests/golden/sass_before_*.json``):
-  - the staged-epilogue 128 x 256 GEMM (``csrc/gemm_wide_sm90.cu`` -> ``fms_fsdp_b200/_gemm_wide.so``), checked by
-    ``tests/test_gemm_epilogue_gpu.py``;
-  - the z-loss kernels (``csrc/losses_sm90.cu`` -> ``fms_fsdp_b200/_losses.so``), checked by ``tests/test_z_loss_gpu.py``.
+* the .so stays in the tree (git-ignored), next to the package, so the package imports from the source tree.
 """
 from __future__ import annotations
 
@@ -26,12 +21,6 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "..", "build", "sm90_ext")
 OUT = os.path.join(HERE, "_C.so")
-WIDE_SRC = "gemm_wide_sm90.cu"
-WIDE_OUT = os.path.join(HERE, "_gemm_wide.so")
-# (source, library, link log) of every side library, in the order _C.so links them
-SIDE_LIBS = [(WIDE_SRC, WIDE_OUT, "link_wide.log"),
-             ("losses_sm90.cu", os.path.join(HERE, "_losses.so"), "link_losses.log")]
-SIDE_SRCS = [src for src, _, _ in SIDE_LIBS]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 CXX = os.environ.get("CXX", "g++")
 
@@ -62,19 +51,18 @@ def build(force: bool = False, verbose: bool = True) -> str:
 
     os.makedirs(BUILD, exist_ok=True)
     headers = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
-    cus = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu") and f not in SIDE_SRCS)
+    cus = sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith(".cu"))
     cpp = os.path.join(CSRC, "bindings.cpp")
     hdr_digest = _digest(headers, " ".join(NVCC_FLAGS) + torch.__version__)
 
     jobs = []
     objs = []
-    for src in [os.path.join(CSRC, f) for f in SIDE_SRCS] + cus + [cpp]:
+    for src in cus + [cpp]:
         base = os.path.basename(src)
         obj = os.path.join(BUILD, base + ".o")
         stamp = obj + ".sha"
         want = _digest([src], hdr_digest)
-        if base not in SIDE_SRCS:
-            objs.append(obj)
+        objs.append(obj)
         have = open(stamp).read() if os.path.exists(stamp) else ""
         if force or have != want or not os.path.exists(obj):
             if src.endswith(".cu"):
@@ -104,15 +92,8 @@ def build(force: bool = False, verbose: bool = True) -> str:
                     print(f"[build] compiled {base}", flush=True)
     tlib = os.path.join(os.path.dirname(torch.__file__), "lib")
     cuda_lib = "/usr/local/cuda/lib64"
-    side_outs = [out for _, out, _ in SIDE_LIBS]
-    if jobs or force or not all(os.path.exists(p) for p in side_outs + [OUT]):
-        for src, lib, log in SIDE_LIBS:
-            cmd = [CXX, "-shared", "-o", lib, os.path.join(BUILD, src + ".o"), "-Wl,-soname," + os.path.basename(lib),
-                   f"-L{cuda_lib}", "-lcudart", f"-Wl,-rpath,{cuda_lib}"]
-            _run(cmd, os.path.join(BUILD, log))
-            if verbose:
-                print(f"[build] linked {lib}", flush=True)
-        cmd = [CXX, "-shared", "-o", OUT] + objs + side_outs + ["-Wl,-rpath,$ORIGIN",
+    if jobs or force or not os.path.exists(OUT):
+        cmd = [CXX, "-shared", "-o", OUT] + objs + [
             f"-L{tlib}", f"-L{cuda_lib}", "-lc10", "-lc10_cuda", "-ltorch_cpu", "-ltorch_cuda", "-ltorch",
             "-ltorch_python", "-lcudart", f"-Wl,-rpath,{tlib}", f"-Wl,-rpath,{cuda_lib}"]
         _run(cmd, os.path.join(BUILD, "link.log"))

@@ -98,7 +98,7 @@ DECL int b200_moe_combine_bwd(const void*, const void*, const float*, const int*
                               int, int, void*, float*, cudaStream_t);
 DECL int b200_moe_route_bwd(const float*, const int*, const float*, const float*, const int*, int, int, int, int, float,
                             void*, cudaStream_t);
-// z-loss kernels (csrc/losses_sm90.cu, fms_fsdp_b200/_losses.so)
+// z-loss kernels (csrc/losses_sm90.cu)
 DECL int b200_ce_zloss_grad_inplace(void*, const long long*, const float*, float*, int, int, int, long long, float,
                                     cudaStream_t);
 DECL int b200_loss_partials_reduce(const float*, int, int, const float*, float, float*, cudaStream_t);

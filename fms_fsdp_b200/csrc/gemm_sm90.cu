@@ -15,10 +15,8 @@
 // Warp roles (384 threads): warpgroup 0 = producer (warp 0 lane 0 issues TMA; warps 2-3 are the comm warps of the fused
 // all-gather), warpgroups 1-2 = consumers (wgmma + epilogue).
 //
-// gemm_wide_bf16 is the same pipeline on a 128 x 256 tile (wgmma m64n256k16) for the GEMMs without fused communication;
-// use_wide picks the tile per launch.  Wherever TMA can describe its operands, the 128 x 256 tile runs with an epilogue
-// staged in shared memory instead (csrc/gemm_wide_sm90.cu); gemm_wide_bf16 serves the other operands and is the
-// bitwise reference.
+// The GEMMs without fused communication may run on a 128 x 256 tile instead (csrc/gemm_wide_sm90.cu); use_wide picks
+// the tile per launch.  Operands TMA cannot describe for that tile's staged epilogue run on the 128 x 128 tile.
 //
 // The operands of the fused epilogues (RoPE table and bias, SwiGLU aux, push table) come with each launch in a
 // GemmEpilogueArgs (gemm_epilogue.h); check_epilogue validates them for all three launch entries.
@@ -141,8 +139,8 @@ B200_DEVINL void epi_pair(const GemmParams& p, OutT* crow, int row, int col, flo
   store2(crow + col, f0, f1);
 }
 
-// Register epilogue of one consumer warpgroup's 64-row slice of a tile that is 8 * NJ columns wide (NJ = 16: 128x128
-// kernel, 32: 128x256 kernel) in tile column nt.  The thread holds rows rbase and rbase + 8, column pairs 8 j + cq for
+// Register epilogue of one consumer warpgroup's 64-row slice of a tile that is 8 * NJ columns wide (NJ = BN / 8 = 16)
+// in tile column nt.  The thread holds rows rbase and rbase + 8, column pairs 8 j + cq for
 // j < NJ.  EPI_SWIGLU: the tile holds gate and up of 4 * NJ features side by side.
 template <int EPI, typename OutT, int NJ>
 B200_DEVINL void epilogue_tile(const GemmParams& p, const float (&acc)[4 * NJ], size_t boff, int rbase, int nt, int cq) {
@@ -451,134 +449,8 @@ static int launch(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmPara
   return (int)cudaGetLastError();
 }
 
-// ---- 128 x 256 tile ("wide"), for the GEMMs without fused communication.  The same pipeline with twice the B tile per
-// stage: a k-block moves 48 KiB for 4.2 MFLOP (85 FLOP per byte from L2, against 64 for 128 x 128), and each consumer
-// warpgroup issues m64n256k16, which reads 10 KiB of shared-memory operands per 524k FLOP where two m64n128k16 read
-// 12 KiB.  A 64 x 256 fp32 accumulator is 128 registers per consumer thread, more than 384 threads get by default:
-// setmaxnreg hands the producer warpgroup's registers to the consumers (128 x 40 + 256 x 232 <= 64K).
-// Epilogues: store, +residual, accumulate (bf16 or fp32 output), RoPE (with or without bias), SwiGLU forward
-// (F % 128 == 0) and backward.
-constexpr int W_SMEM_BYTES = W_STAGES * W_STAGE_BYTES + 1024 + 256;
-
-template <bool A_MN, bool B_MN, int EPI, typename OutT>
-__global__ void __launch_bounds__(THREADS, 1)
-gemm_wide_bf16(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + W_STAGES * W_STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + W_STAGES;
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_kb = (p.K + BK - 1) / BK;
-  const int num_tiles = p.m_tiles * p.n_tiles;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int s = 0; s < W_STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 8);   // one arrive per consumer warp
-    }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp < 4) {
-    setmaxnreg_dec<40>();
-    if (warp == 0 && lane == 0) {
-      // ============================== TMA producer ==============================
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int mt, nt;
-        tile_coords(t, p.m_tiles, p.n_tiles, mt, nt);
-        const int m0 = mt * BM;
-        // first B row (K-major) or column (MN-major) of the tile; SwiGLU: 128 features of the first half of the fused
-        // weight in B rows [f0, f0 + 128), the same features of the second half in [F + f0, F + f0 + 128)
-        const int n0 = (EPI == EPI_SWIGLU) ? nt * 128 : nt * WBN;
-        const int n2 = (EPI == EPI_SWIGLU) ? n0 + p.swi_F : n0 + 128;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * W_STAGE_BYTES;
-          uint8_t* sb = sa + A_BYTES;
-          const int k0 = kb * BK;
-          mbar_arrive_expect_tx(&full_bar[stage], W_STAGE_BYTES);
-          if constexpr (!A_MN) {
-            tma_load_2d(sa, &tmA, &full_bar[stage], k0, m0);                     // box {64 k, 128 rows}
-          } else {
-            tma_load_2d(sa, &tmA, &full_bar[stage], m0, k0);                     // boxes {64 m, 64 k-rows}
-            tma_load_2d(sa + 64 * BK * 2, &tmA, &full_bar[stage], m0 + 64, k0);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {                                            // four 64-wide quarters of B
-            const int nq = (q < 2 ? n0 : n2) + 64 * (q & 1);
-            if constexpr (!B_MN) tma_load_2d(sb + q * 64 * BK * 2, &tmB, &full_bar[stage], k0, nq);
-            else                 tma_load_2d(sb + q * 64 * BK * 2, &tmB, &full_bar[stage], nq, k0);
-          }
-          if (++stage == W_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    setmaxnreg_inc<232>();
-    // ============================== consumers: wgmma + epilogue ==============================
-    const int cw = (warp >> 2) - 1;          // consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile
-    const int w4 = warp & 3;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int mt, nt;
-      tile_coords(t, p.m_tiles, p.n_tiles, mt, nt);
-      float acc[128];
-#pragma unroll
-      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_u32(smem + stage * W_STAGE_BYTES) + cw * (64 * 128);
-        const uint32_t sb = smem_u32(smem + stage * W_STAGE_BYTES) + A_BYTES;
-        const uint64_t a0 = make_smem_desc(sa, 0, 1024);
-        const uint64_t bd0 = make_smem_desc(sb, B_MN ? 64 * BK * 2 : 0, 1024);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t adesc = a0 + ((A_MN ? k * 2048 : k * 32) >> 4);
-          const uint64_t bdesc = bd0 + ((B_MN ? k * 2048 : k * 32) >> 4);
-          wgmma_bf16_ss_n256<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, adesc, bdesc, (kb | k) != 0);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                     // the previous k-block's MMAs have retired: release its stage
-        if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-        prev = stage;
-        if (++stage == W_STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      const int rbase = mt * BM + cw * 64 + w4 * 16 + (lane >> 2);
-      epilogue_tile<EPI, OutT, WBN / 8>(p, acc, 0, rbase, nt, 2 * (lane & 3));
-    }
-  }
-}
-
-template <bool A_MN, bool B_MN, int EPI, typename OutT>
-static int launch_wide(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
-  auto kern = gemm_wide_bf16<A_MN, B_MN, EPI, OutT>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM_BYTES);
-    if (e != cudaSuccess) return (int)e;
-    configured = true;
-  }
-  p.n_tiles = (EPI == EPI_SWIGLU) ? p.swi_F / 128 : (p.N + WBN - 1) / WBN;
-  const long long tiles = (long long)p.m_tiles * p.n_tiles;
-  const int grid = tiles < sm_count() ? (int)tiles : sm_count();
-  kern<<<grid, THREADS, W_SMEM_BYTES, stream>>>(tmA, tmB, p);
-  return (int)cudaGetLastError();
-}
-
-// 0: the launcher picks the tile; 1: always 128 x 128; 2: 128 x 256 wherever the epilogue allows it; 3: as 2, with the
-// register epilogue (gemm_wide_bf16) instead of the staged one.  Set only by the GEMM benchmark and the tests, which
-// compare the tiles and epilogues on the same operands.
+// 0: the launcher picks the tile; 1: always 128 x 128; 2: 128 x 256 wherever the epilogue and the operands allow it.
+// Set only by the GEMM benchmark and the tests, which compare the tiles on the same operands.
 static int g_tile_override = 0;
 
 // The wide tile moves less data per FLOP but halves the tile count, so it wins unless it leaves a worse last wave:
@@ -596,15 +468,12 @@ static bool use_wide(const GemmParams& p, int epi) {
 }
 
 // every GEMM of the single-GPU path (no fused all-gather, no push): one launch of the tile use_wide picks.  The
-// 128 x 256 tile runs with the staged epilogue (csrc/gemm_wide_sm90.cu) wherever TMA can describe its operands.
+// 128 x 256 tile (csrc/gemm_wide_sm90.cu) takes only operands TMA can describe; the others run on the 128 x 128 tile.
 template <bool A_MN, bool B_MN, int EPI, typename OutT>
 static int launch_local(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmParams& p, cudaStream_t stream) {
-  if (use_wide(p, EPI)) {
-    constexpr int fp32 = sizeof(OutT) == 4;
-    if (g_tile_override != 3 && b200_gemm_wide_staged_ok(&p, EPI, fp32))
-      return b200_gemm_wide_staged(&tmA, &tmB, &p, A_MN, B_MN, EPI, fp32, stream);
-    return launch_wide<A_MN, B_MN, EPI, OutT>(tmA, tmB, p, stream);
-  }
+  constexpr int fp32 = sizeof(OutT) == 4;
+  if (use_wide(p, EPI) && b200_gemm_wide_staged_ok(&p, EPI, fp32))
+    return b200_gemm_wide_staged(&tmA, &tmB, &p, A_MN, B_MN, EPI, fp32, stream);
   return launch<A_MN, B_MN, EPI, OutT, false>(tmA, tmB, p, AgParams{}, stream);
 }
 
@@ -696,8 +565,8 @@ static int check_epilogue(const GemmEpilogueArgs& e, int epi, int N, int ldc, in
 
 }  // namespace b200
 
-// tile of the single-GPU GEMMs: 0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256 where the epilogue allows it
-extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode >= 1 && mode <= 3) ? mode : 0; }
+// tile of the single-GPU GEMMs: 0 = chosen per launch, 1 = 128 x 128, 2 = 128 x 256 where the epilogue and operands allow it
+extern "C" void b200_gemm2_set_tile(int mode) { b200::g_tile_override = (mode >= 1 && mode <= 2) ? mode : 0; }
 
 // C[M,N] = op(A) op(B) (+R | +C | fused epilogue).  a_mn: A is stored [K,M] (M contiguous) else [M,K];  b_mn: B is
 // stored [K,N] (N contiguous) else [N,K].  lda/ldb/ldc/ldr are row strides in elements.  Returns 0 or an error code.

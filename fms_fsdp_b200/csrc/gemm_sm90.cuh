@@ -1,4 +1,4 @@
-// Definitions shared by the GEMM kernels of csrc/gemm_sm90.cu and the staged-epilogue 128 x 256 GEMM of
+// Definitions shared by the 128 x 128 GEMM kernels of csrc/gemm_sm90.cu and the 128 x 256 GEMM of
 // csrc/gemm_wide_sm90.cu: tile constants, epilogue codes, the launch parameters and the per-element helpers.
 #pragma once
 #include "common.cuh"
@@ -93,19 +93,12 @@ B200_DEVINL float2 load2(const OutT* p) {
   else return *reinterpret_cast<const float2*>(p);
 }
 
-constexpr int WBN = 256;
-constexpr int W_STAGES = 4;
-constexpr int W_STAGE_BYTES = A_BYTES + WBN * BK * 2;   // 16 + 32 KiB
-
-template <int N>
-B200_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N>
-B200_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+constexpr int WBN = 256;                      // columns of the 128 x 256 tile
 
 }  // namespace b200
 
-// The 128 x 256 tile with the staged epilogue (csrc/gemm_wide_sm90.cu, library _gemm_wide.so).  _ok: 1 when TMA can
-// describe the epilogue's operands (16-byte aligned bases and row strides, no row stride below the row).
+// The 128 x 256 tile (csrc/gemm_wide_sm90.cu).  _ok: 1 when the tile has the epilogue (all but fp32 +residual) and TMA
+// can describe its operands (16-byte aligned bases and row strides, no row stride below the row).
 extern "C" int b200_gemm_wide_staged_ok(const b200::GemmParams* p, int epi, int out_fp32);
 extern "C" int b200_gemm_wide_staged(const CUtensorMap* tmA, const CUtensorMap* tmB, const b200::GemmParams* p,
                                      int a_mn, int b_mn, int epi, int out_fp32, cudaStream_t stream);

@@ -1,14 +1,18 @@
-// The 128 x 256 GEMM tile of csrc/gemm_sm90.cu (gemm_wide_bf16: same producer, ring and main loop) with its epilogue
-// staged in shared memory.  Built as a library of its own (fms_fsdp_b200/_gemm_wide.so, see build.py) that _C.so links:
-// the launcher in gemm_sm90.cu calls b200_gemm_wide_staged for every 128 x 256 GEMM whose operands TMA can describe,
-// and keeps the register-epilogue kernel for the others and as the bitwise reference.
+// The 128 x 256 GEMM tile: the pipeline of the 128 x 128 kernel in csrc/gemm_sm90.cu with twice the B tile per stage,
+// and an epilogue staged in shared memory.  The launcher in gemm_sm90.cu calls b200_gemm_wide_staged for the 128 x 256
+// GEMMs whose operands TMA can describe; the others run on the 128 x 128 tile.
+//
+// A k-block moves 48 KiB for 4.2 MFLOP (85 FLOP per byte from L2, against 64 for 128 x 128), and each consumer
+// warpgroup issues m64n256k16, which reads 10 KiB of shared-memory operands per 524k FLOP where two m64n128k16 read
+// 12 KiB.  A 64 x 256 fp32 accumulator is 128 registers per consumer thread, more than 384 threads get by default:
+// setmaxnreg hands the producer warpgroup's registers to the consumers (128 x 40 + 256 x 232 <= 64K).
 //
 // Each consumer warpgroup walks its 64 x 256 slice in 32-column subtiles, writes each result block ("slab", 64 rows x
 // 32 columns of one output) into a swizzled staging buffer and one thread sends it with a TMA tensor store, which clips
 // at the M and N edges.  The epilogue operands (residual, the C that is accumulated into, the saved SwiGLU projection)
 // arrive by TMA loads into the same slabs, the first ones while the main loop's last k-blocks run and the next ones
 // while a subtile is computed; each result is written in place over its operand.  The arithmetic per element is that
-// of epi_pair / epilogue_tile in gemm_sm90.cu, so every tile gives the same bits.
+// of epi_pair / epilogue_tile in gemm_sm90.cu, so both tiles give the same bits.
 // Epilogues: store, +residual (bf16 output), accumulate (bf16 or fp32 output), RoPE (with or without bias), SwiGLU
 // forward (F % 128 == 0) and backward.
 #include "common.cuh"
@@ -18,6 +22,8 @@
 
 namespace b200 {
 
+constexpr int W_STAGES = 4;
+constexpr int W_STAGE_BYTES = A_BYTES + WBN * BK * 2;   // 16 + 32 KiB
 constexpr int W_SUB = 32;                               // columns per epilogue subtile
 constexpr int W_STG_BYTES = 16384;                      // epilogue staging per consumer warpgroup
 constexpr int W_SMEM_BYTES = W_STAGES * W_STAGE_BYTES + 2 * W_STG_BYTES + 1024 + 256;
@@ -46,6 +52,11 @@ struct WideEpi {
 struct WideEpiMaps {
   CUtensorMap c, c2, x, x2;
 };
+
+template <int N>
+B200_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+B200_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 // byte offset of element (r, c) in a slab
 template <typename OutT>
@@ -402,7 +413,7 @@ static int dispatch_staged(const CUtensorMap& a, const CUtensorMap& b, const Gem
 
 extern "C" int b200_gemm_wide_staged_ok(const b200::GemmParams* p, int epi, int out_fp32) {
   using namespace b200;
-  if (out_fp32 && epi != EPI_STORE && epi != EPI_ACCUM) return 0;   // fp32 +residual: register epilogue
+  if (out_fp32 && epi != EPI_STORE && epi != EPI_ACCUM) return 0;   // fp32 +residual: 128 x 128 tile
   return staged_ok(*p, epi, out_fp32 ? 4 : 2) ? 1 : 0;
 }
 

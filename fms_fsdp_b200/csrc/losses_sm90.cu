@@ -1,9 +1,8 @@
 // Auxiliary stability losses fused into the kernels that already hold the softmax normaliser (sm_90a):
 //   * output z-loss  c * mean_t lse_t^2 inside the softmax cross-entropy gradient of a logits chunk;
 //   * router z-loss  c_r * mean_t (logsumexp_e router_logits_te)^2 of the mixture-of-experts routing.
-// A library of its own (fms_fsdp_b200/_losses.so, which _C.so links), so the kernels of _C.so keep the instructions
-// their recorded digests pin.  Every statistic goes to per-row or per-CTA fp32 partials that one CTA sums in a fixed
-// order: no float atomics, so gradients and statistics are the same bits on every run.
+// Every statistic goes to per-row or per-CTA fp32 partials that one CTA sums in a fixed order: no float atomics, so
+// gradients and statistics are the same bits on every run.
 #include "common.cuh"
 
 namespace b200 {

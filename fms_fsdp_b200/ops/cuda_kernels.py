@@ -579,7 +579,7 @@ def cross_entropy_fwd_bwd(logits, labels, ignore_index=-100):
     return loss_sum / n_valid.clamp(min=1.0), g
 
 
-# ------------------------------------------------------------------- z-loss (csrc/losses_sm90.cu, _losses.so)
+# ------------------------------------------------------------------------------- z-loss (csrc/losses_sm90.cu)
 def linear_ce_z_fwd_bwd(h, w, labels, dw_out, z_coef, ignore_index=-100, chunk_rows=4096, accumulate=False):
     """(CE, z, dh): ``linear_ce_fwd_bwd`` with the output z-loss inside the gradient kernel.  Each row's CE and lse^2
     go to a per-row partial; one CTA sums them in a fixed order (the same bits on every run)."""

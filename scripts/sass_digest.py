@@ -1,9 +1,10 @@
 """Per-kernel SHA-256 digests of the SASS instructions of the built extension (addresses and encodings stripped):
 
-    python scripts/sass_digest.py [fms_fsdp_b200/_C.so] > tests/golden/sass_before_qk_norm.json
+    python scripts/sass_digest.py [fms_fsdp_b200/_C.so] > tests/golden/sass_kernels.json
 
-A pull request that must leave existing kernels byte-identical compares these digests before and after
-(``tests/test_qk_norm_gpu.py``)."""
+``tests/test_sass.py`` holds every kernel of ``_C.so`` to ``tests/golden/sass_kernels.json``.  A change that means to
+change, add or remove kernels regenerates that file with this script in the same commit, so that the JSON diff names
+every kernel whose instructions changed."""
 import hashlib
 import json
 import os
@@ -11,11 +12,13 @@ import re
 import subprocess
 import sys
 
+CUOBJDUMP = "/usr/local/cuda/bin/cuobjdump"
 
-def digests(so):
-    out = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-sass", so], capture_output=True, text=True, check=True).stdout
+
+def parse(sass):
+    """{kernel: [instruction text]} of a ``cuobjdump -sass`` listing, without addresses and encodings."""
     per, name = {}, None
-    for line in out.splitlines():
+    for line in sass.splitlines():
         m = re.search(r"Function : (\S+)", line)
         if m:
             name = m.group(1)
@@ -24,10 +27,15 @@ def digests(so):
         m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)
         if name and m:
             per[name].append(m.group(1))
+    return per
+
+
+def digests(per):
     return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in sorted(per.items())}
 
 
 if __name__ == "__main__":
     so = sys.argv[1] if len(sys.argv) > 1 else os.path.join(os.path.dirname(__file__), "..", "fms_fsdp_b200", "_C.so")
-    json.dump(digests(so), sys.stdout, indent=0, sort_keys=True)
+    out = subprocess.run([CUOBJDUMP, "-sass", so], capture_output=True, text=True, check=True).stdout
+    json.dump(digests(parse(out)), sys.stdout, indent=0, sort_keys=True)
     sys.stdout.write("\n")

@@ -1,12 +1,8 @@
 """GPU tier: the warp-specialised attention kernels (``attn_fwd_pipe_kernel`` / ``attn_bwd_pipe_kernel``) against the
 fp32 oracle and bit for bit against the lock-step kernels they replace, where the producer ring wraps or runs short
 (1-5 streamed tiles against a ring of 2 / 3 stages), on ragged sequences, every GQA group size and document layouts with
-1-, 64- and 513-token documents; run-to-run determinism at the headline shape; and the SASS of the new kernels."""
-import json
-import os
-import re
-import shutil
-import subprocess
+1-, 64- and 513-token documents; and run-to-run determinism at the headline shape.  ``tests/test_sass.py`` checks their
+SASS."""
 
 import pytest
 import torch
@@ -15,7 +11,6 @@ from fms_fsdp_b200 import ops
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SEP = 1
 
 
@@ -125,59 +120,3 @@ def test_headline_shape_bitwise_lockstep_and_deterministic(K, H, KVH):
     _assert_bitwise(new, ref)
     again, _ = _both(CK, qkv, do, B, S, H, KVH, hd)
     _assert_bitwise(again, new)
-
-
-# --------------------------------------------------------------------------------------------------------- SASS
-def _sass():
-    so = os.path.join(ROOT, "fms_fsdp_b200", "_C.so")
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(so) or not os.path.exists(exe):
-        pytest.skip("needs the built extension and cuobjdump")
-    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
-    import hashlib
-    per, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            per[name] = []
-            continue
-        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)      # instruction lines only, without addresses
-        if name and m:
-            per[name].append(m.group(1))
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in per.items()}, per
-
-
-# The atomic embedding backward was later replaced by the sorted fixed-order sum (tests/test_llama_kernels_gpu.py checks
-# its kernels); these four kernels are expected to be gone.
-EMBEDDING_BWD_REPLACED = {
-    "_ZN4b20020embedding_bwd_kernelIiEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20020embedding_bwd_kernelIxEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20024embedding_bwd_f32_kernelIiEEvPKT_PK13__nv_bfloat16Pfmi",
-    "_ZN4b20024embedding_bwd_f32_kernelIxEEvPKT_PK13__nv_bfloat16Pfmi",
-}
-
-
-def test_sass_pipelined_kernels_and_existing_kernels_unchanged_but_the_embedding_backward():
-    """``tests/golden/sass_before_attn_pipeline.json``: per-kernel digests of every kernel of the extension before the
-    pipelined attention kernels were added (``scripts/sass_digest.py``, CUDA 12.9), the lock-step attention kernels
-    included.  setmaxnreg is ``USETMAXREG`` in SASS; the dK/dV instantiations bring -lse / -delta in by ``UBLKCP``."""
-    digests, per = _sass()
-    new = [k for k in per if "attn_fwd_pipe_kernel" in k or "attn_bwd_pipe_kernel" in k]
-    assert len(new) == 4 + 8, new
-    for k in new:
-        body = per[k]
-        assert any(i.startswith("HGMMA") for i in body) and any(i.startswith("UTMALDG") for i in body), k
-        assert sum(i.startswith("USETMAXREG") for i in body) == 2, k          # producer dec + consumer inc
-        assert not any(re.match(r"(LDL|STL)\b", i) for i in body), k
-        # the overlap survives register allocation: a kernel whose wgmmas ptxas serialised (C7512) waits after every
-        # HGMMA; the schedule waits at most 4 times (forward: S, PV in the loop and around it; backward: S, dP, end)
-        depbar = sum(i.startswith("WARPGROUP.DEPBAR") for i in body)
-        hgmma = sum(i.startswith("HGMMA") for i in body)
-        assert depbar <= 4 and 3 * depbar <= hgmma, (k, depbar, hgmma)
-        if "attn_bwd_pipe_kernelILi128ELi0E" in k or "attn_bwd_pipe_kernelILi64ELi0E" in k:
-            assert any(i.startswith("UBLKCP") for i in body), k
-    with open(os.path.join(ROOT, "tests", "golden", "sass_before_attn_pipeline.json")) as f:
-        before = json.load(f)
-    changed = [k for k, v in before.items() if digests.get(k) != v and k not in EMBEDDING_BWD_REPLACED]
-    assert not changed, changed

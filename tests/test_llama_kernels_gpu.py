@@ -8,12 +8,6 @@ Errors are max-abs over the reference's max-abs, row by row for [M, D] outputs (
 call must launch our kernels and take no ATen fallback, except where a test asserts the counted fallback.
 ``tests/test_llama_kernels_cpu.py`` pins the references and shows each probe fails on a plausible bug.
 """
-import hashlib
-import json
-import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
@@ -21,7 +15,6 @@ import torch
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 F64 = torch.float64
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 # about 3x the largest error measured on an H100 80GB HBM3 at 700 W (DESIGN.md); tests/test_llama_kernels_cpu.py keeps a
 # copy.  bf16 outputs sit near half a bf16 ulp (2^-9 = 2e-3) of their row's largest element.  The CE loss, dh and dw are
@@ -443,48 +436,3 @@ def test_sumsq_misaligned_view_takes_the_counted_fallback(K):
     assert CK.fallback_count() == f0 + 1
     ref = x.double().pow(2).sum()
     check("sumsq misaligned", abs(s.item() - ref.item()) / ref.item(), TOL_SUMSQ)
-
-
-# --------------------------------------------------------------------------------------------------------- SASS
-REPLACED = {                                    # the atomic embedding backward, replaced by the fixed-order sum
-    "_ZN4b20020embedding_bwd_kernelIiEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20020embedding_bwd_kernelIxEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20024embedding_bwd_f32_kernelIiEEvPKT_PK13__nv_bfloat16Pfmi",
-    "_ZN4b20024embedding_bwd_f32_kernelIxEEvPKT_PK13__nv_bfloat16Pfmi",
-}
-
-
-def _sass():
-    so = os.path.join(ROOT, "fms_fsdp_b200", "_C.so")
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(so) or not os.path.exists(exe):
-        pytest.skip("needs the built extension and cuobjdump")
-    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
-    per, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            per[name] = []
-            continue
-        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)      # instruction lines only, without addresses
-        if name and m:
-            per[name].append(m.group(1))
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in per.items()}, per
-
-
-def test_sass_embedding_backward_kernels_no_local_memory_and_every_other_kernel_unchanged():
-    """``tests/golden/sass_before_embedding_sum.json``: per-kernel digests of every kernel of the extension before the
-    embedding backward was replaced (``scripts/sass_digest.py``, CUDA 12.9).  The four atomic kernels are gone, the seven
-    new ones (sort tile and merge, segmented sum and combine for bf16 and fp32 gradients) use no local memory, and every
-    other kernel compiles to the same instructions."""
-    digests, per = _sass()
-    with open(os.path.join(ROOT, "tests", "golden", "sass_before_embedding_sum.json")) as f:
-        before = json.load(f)
-    assert not REPLACED & set(per) and REPLACED <= set(before)
-    new = sorted(k for k in per if k not in before)
-    assert len(new) == 7 and all(re.search(r"embedding_(sort_tile|merge|seg_sum|seg_combine)_kernel", k) for k in new), new
-    for k in new:
-        assert not any(re.match(r"(LDL|STL)\b", i) for i in per[k]), k
-    changed = [k for k, v in before.items() if k not in REPLACED and digests.get(k) != v]
-    assert not changed, changed

@@ -1,10 +1,5 @@
 """Mixture of experts on the GPU: every kernel of ``csrc/moe.cu`` and every grouped GEMM mode against the ATen oracle,
-run-to-run bit reproducibility, no host synchronisation, and the SASS of the new and the existing kernels."""
-import json
-import os
-import re
-import shutil
-import subprocess
+run-to-run bit reproducibility and no host synchronisation.  ``tests/test_sass.py`` checks their SASS."""
 
 import pytest
 import torch
@@ -13,7 +8,6 @@ from fms_fsdp_b200 import ops
 from fms_fsdp_b200.ops import torch_kernels as tk
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -250,52 +244,3 @@ def test_allocator_peak_of_a_4_layer_qwen3_moe_matches_the_memory_plan(ck):
     plan = plan_llama("qwen3_moe_30b_a3b", gpus=1, batch_size=2, seq_length=4096, nlayers=4).total_gib
     print(f"allocator peak {peak:.3f} GiB, plan {plan:.3f} GiB")
     assert abs(peak - plan) / plan < 0.005, (peak, plan)
-
-
-def _sass():
-    so = os.path.join(ROOT, "fms_fsdp_b200", "_C.so")
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(so) or not os.path.exists(exe):
-        pytest.skip("needs the built extension and cuobjdump")
-    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
-    import hashlib
-    per, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            per[name] = []
-            continue
-        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)
-        if name and m:
-            per[name].append(m.group(1))
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in per.items()}, per
-
-
-# The atomic embedding backward was later replaced by the sorted fixed-order sum (tests/test_llama_kernels_gpu.py checks
-# its kernels); these four kernels are expected to be gone.
-EMBEDDING_BWD_REPLACED = {
-    "_ZN4b20020embedding_bwd_kernelIiEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20020embedding_bwd_kernelIxEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20024embedding_bwd_f32_kernelIiEEvPKT_PK13__nv_bfloat16Pfmi",
-    "_ZN4b20024embedding_bwd_f32_kernelIxEEvPKT_PK13__nv_bfloat16Pfmi",
-}
-
-
-def test_sass_grouped_kernels_and_existing_kernels_unchanged_but_the_embedding_backward():
-    """``tests/golden/sass_before_moe.json``: per-kernel digests of every kernel of the extension before the MoE kernels
-    were added (``scripts/sass_digest.py``, CUDA 12.9).  Grouped GEMM instantiations carry GRP_M (16) or GRP_K (32) in
-    their EPI argument."""
-    digests, per = _sass()
-    grouped = [k for k in per if re.search(r"gemm_bf16_wgmmaILb[01]ELb[01]ELi(1[6-9]|2\d|3\d|4\d)E", k)]
-    assert len(grouped) == 8, grouped
-    for k in grouped:
-        assert any("HGMMA" in i for i in per[k]) and any("UTMALDG" in i for i in per[k]), k
-    new = grouped + [k for k in per if "moe_" in k]
-    assert len(new) == 8 + 9, new
-    for k in new:
-        assert not any(re.match(r"(LDL|STL)\b", i) for i in per[k]), k
-    with open(os.path.join(ROOT, "tests", "golden", "sass_before_moe.json")) as f:
-        before = json.load(f)
-    changed = [k for k, v in before.items() if digests.get(k) != v and k not in EMBEDDING_BWD_REPLACED]
-    assert not changed, changed

@@ -1,11 +1,6 @@
 """GPU tier: the QK-norm kernels (``qk_norm_rope`` / ``qk_norm_bwd``) against the fp32 oracle, their determinism,
 ``qkv_attention(qk_norm=...)`` on the fused kernels against the ATen path (plain, document-masked and fp8), one engine step
-of a Qwen3-1.7B-shaped model, and the SASS of the new kernels."""
-import json
-import os
-import re
-import shutil
-import subprocess
+of a Qwen3-1.7B-shaped model.  ``tests/test_sass.py`` checks their SASS."""
 
 import pytest
 import torch
@@ -14,7 +9,6 @@ from fms_fsdp_b200 import ops
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -176,48 +170,3 @@ def test_engine_step_qwen3_shape_fused_matches_aten_path():
         assert abs(lf - la) < 2e-2 * abs(la) and abs(gf - ga) < 5e-2 * abs(ga)
     assert not torch.equal(qf, torch.ones_like(qf))          # the norm gains were trained
     assert (qf - qa).abs().max() < 2e-3
-
-
-# --------------------------------------------------------------------------------------------------------- SASS
-def _sass():
-    so = os.path.join(ROOT, "fms_fsdp_b200", "_C.so")
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(so) or not os.path.exists(exe):
-        pytest.skip("needs the built extension and cuobjdump")
-    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
-    import hashlib
-    per, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            per[name] = []
-            continue
-        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)      # instruction lines only, without addresses
-        if name and m:
-            per[name].append(m.group(1))
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in per.items()}, per
-
-
-# The atomic embedding backward was later replaced by the sorted fixed-order sum (tests/test_llama_kernels_gpu.py checks
-# its kernels); these four kernels are expected to be gone.
-EMBEDDING_BWD_REPLACED = {
-    "_ZN4b20020embedding_bwd_kernelIiEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20020embedding_bwd_kernelIxEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20024embedding_bwd_f32_kernelIiEEvPKT_PK13__nv_bfloat16Pfmi",
-    "_ZN4b20024embedding_bwd_f32_kernelIxEEvPKT_PK13__nv_bfloat16Pfmi",
-}
-
-
-def test_sass_new_kernels_no_local_memory_and_existing_kernels_unchanged_but_the_embedding_backward():
-    """``tests/golden/sass_before_qk_norm.json``: per-kernel digests of the instructions of every kernel of the extension as
-    it was before the QK-norm kernels were added (``scripts/sass_digest.py``, CUDA 12.9).  Adding QK-norm changes none."""
-    digests, per = _sass()
-    new = [k for k in per if "qk_norm" in k]
-    assert len(new) == 4, new
-    for k in new:
-        assert not any(re.match(r"(LDL|STL)\b", i) for i in per[k]), k
-    with open(os.path.join(ROOT, "tests", "golden", "sass_before_qk_norm.json")) as f:
-        before = json.load(f)
-    changed = [k for k, v in before.items() if digests.get(k) != v and k not in EMBEDDING_BWD_REPLACED]
-    assert not changed, changed

@@ -1,14 +1,8 @@
 """GPU tier: the q / k / v bias + RoPE epilogue of the QKV GEMM (``EPI_ROPE_BIAS``) on the 128 x 128 tile, the 128 x 256
 tile and the fused all-gather build, ``bias_grad`` against an fp64 column sum and its determinism,
 ``qkv_attention(qkv_bias=...)`` on the fused kernels against the ATen path (plain and document-masked), one engine step of
-a Qwen2.5-1.5B-shaped model, and the SASS of the new kernels."""
+a Qwen2.5-1.5B-shaped model.  ``tests/test_sass.py`` checks their SASS."""
 import contextlib
-import hashlib
-import json
-import os
-import re
-import shutil
-import subprocess
 
 import pytest
 import torch
@@ -17,7 +11,6 @@ from fms_fsdp_b200 import ops
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
@@ -222,50 +215,3 @@ def test_engine_step_qwen25_shape_fused_matches_aten_path():
     # near zero may step the other way on the two paths; nearly all elements must agree to a small part of the step
     d = (bf - ba).abs()
     assert d.median() < 1e-4 and (d < 2e-4).float().mean() > 0.95
-
-
-# --------------------------------------------------------------------------------------------------------- SASS
-def _sass():
-    so = os.path.join(ROOT, "fms_fsdp_b200", "_C.so")
-    exe = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
-    if not os.path.exists(so) or not os.path.exists(exe):
-        pytest.skip("needs the built extension and cuobjdump")
-    out = subprocess.run([exe, "-sass", so], capture_output=True, text=True, timeout=600).stdout
-    per, name = {}, None
-    for line in out.splitlines():
-        m = re.search(r"Function : (\S+)", line)
-        if m:
-            name = m.group(1)
-            per[name] = []
-            continue
-        m = re.match(r"\s*/\*[0-9a-f]{4,}\*/\s+(.*?;)", line)      # instruction lines only, without addresses
-        if name and m:
-            per[name].append(m.group(1))
-    return {k: hashlib.sha256("\n".join(v).encode()).hexdigest() for k, v in per.items()}, per
-
-
-# The atomic embedding backward was later replaced by the sorted fixed-order sum (tests/test_llama_kernels_gpu.py checks
-# its kernels); these four kernels are expected to be gone.
-EMBEDDING_BWD_REPLACED = {
-    "_ZN4b20020embedding_bwd_kernelIiEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20020embedding_bwd_kernelIxEEvPKT_PK13__nv_bfloat16PS4_mi",
-    "_ZN4b20024embedding_bwd_f32_kernelIiEEvPKT_PK13__nv_bfloat16Pfmi",
-    "_ZN4b20024embedding_bwd_f32_kernelIxEEvPKT_PK13__nv_bfloat16Pfmi",
-}
-
-
-def test_sass_new_kernels_no_local_memory_and_existing_kernels_unchanged_but_the_embedding_backward():
-    """``tests/golden/sass_before_qkv_bias.json``: per-kernel digests of the instructions of every kernel of the extension
-    as it was before the bias epilogue and ``bias_grad`` were added (``scripts/sass_digest.py``, CUDA 12.9).  Adding them
-    changes none."""
-    digests, per = _sass()
-    with open(os.path.join(ROOT, "tests", "golden", "sass_before_qkv_bias.json")) as f:
-        before = json.load(f)
-    new = sorted(k for k in per if k not in before
-                 and not re.search(r"embedding_(sort_tile|merge|seg_sum|seg_combine)_kernel", k))
-    # EPI_ROPE_BIAS = 8 in the 128 x 128 kernel (plain and all-gather builds) and the 128 x 256 kernel, and bias_grad
-    assert len(new) == 4 and sum("Li8E" in k for k in new) == 3 and any("bias_grad" in k for k in new), new
-    for k in new:
-        assert not any(re.match(r"(LDL|STL)\b", i) for i in per[k]), k
-    changed = [k for k, v in before.items() if digests.get(k) != v and k not in EMBEDDING_BWD_REPLACED]
-    assert not changed, changed
