@@ -1261,7 +1261,11 @@ extern "C" int b200_bias_grad(const void* dy, float* part, float* db, int T, int
 
 // ------------------------------------------------------------------------------------------------------------------
 // Row-wise e4m3 quantisation for the optional fp8 forward GEMMs: one warp per row; scale[row] = amax(row) / 448 (the
-// largest finite e4m3 value), q = x / scale rounded to nearest, saturating.  The second pass re-reads the row from L1/L2.
+// largest finite e4m3 value), q = x / scale rounded to nearest even, saturating.  Both quotients are IEEE divisions
+// (__fdiv_rn, whatever the fast-math flags): amax * (1 / 448.f) or x * (1 / scale) would be off by an ulp for about
+// half the rows and move q across a rounding boundary for about 2 in 10^4 elements
+// (tests/test_gemm_numerics_gpu.py::test_quant_rowwise_e4m3_exact holds both bit for bit).  The second pass re-reads
+// the row from L1/L2.
 namespace b200 {
 B200_DEVINL uint32_t cvt_e4m3x4(float a, float b, float c, float d) {
   uint16_t lo, hi;
@@ -1285,16 +1289,16 @@ __global__ void __launch_bounds__(256) quant_rowwise_e4m3_kernel(const __nv_bflo
     }
   }
   amax = warp_max(amax);
-  const float sc = amax > 0.f ? amax * (1.f / 448.f) : 1.f;
-  const float inv = 1.f / sc;
+  const float sc = amax > 0.f ? __fdiv_rn(amax, 448.f) : 1.f;
   if (lane == 0) scale[row] = sc;
   uint8_t* qr = q + (size_t)row * ldq;
   for (int c = lane * 8; c < K; c += 256) {
     const uint4 v = *reinterpret_cast<const uint4*>(xr + c);
     const float2 a = unpack_bf16x2(v.x), b = unpack_bf16x2(v.y), e = unpack_bf16x2(v.z), f = unpack_bf16x2(v.w);
     uint2 o;
-    o.x = cvt_e4m3x4(a.x * inv, a.y * inv, b.x * inv, b.y * inv);
-    o.y = cvt_e4m3x4(e.x * inv, e.y * inv, f.x * inv, f.y * inv);
+    const auto g = [sc](float x) { return __fdiv_rn(x, sc); };
+    o.x = cvt_e4m3x4(g(a.x), g(a.y), g(b.x), g(b.y));
+    o.y = cvt_e4m3x4(g(e.x), g(e.y), g(f.x), g(f.y));
     *reinterpret_cast<uint2*>(qr + c) = o;
   }
 }

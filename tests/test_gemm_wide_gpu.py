@@ -1,11 +1,13 @@
 """The 128 x 256 GEMM tile (``gemm_wide_staged_bf16`` in csrc/gemm_wide_sm90.cu): every GEMM of the Llama2-1.4B headline step at its
 real shape, layout, epilogue and output dtype, and the edge cases of the tile, against the fp32 oracle and against the
-128 x 128 tile on the same operands.  Both tiles sum each output element over k in the same order (64-wide k-blocks,
+128 x 128 tile on the same operands; every element of both within the float64 bound of tests/gemm_reference.py.  Both tiles sum each output element over k in the same order (64-wide k-blocks,
 k16 MMAs in sequence), so they agree to the last bit."""
 import contextlib
 
 import pytest
 import torch
+
+import gemm_reference as GR
 
 DEV = "cuda"
 T, D, F, H, KVH, HD, V, S = 8192, 2048, 6144, 16, 4, 128, 32000, 4096
@@ -62,50 +64,38 @@ def tile(CK, mode):
         CK._C._set_gemm_tile(0)
 
 
-def tile_rel(out, ref, bm=128, bn=256):
-    """Largest per-tile relative error: max |out - ref| / max |ref| over each bm x bn block."""
-    out, ref = out.float(), ref.float()
-    M, N = ref.shape
-    pm, pn = (-M) % bm, (-N) % bn
-    e = torch.nn.functional.pad((out - ref).abs(), (0, pn, 0, pm))
-    r = torch.nn.functional.pad(ref.abs(), (0, pn, 0, pm))
-    blk = lambda x: x.view((M + pm) // bm, bm, (N + pn) // bn, bn).amax(dim=(1, 3))
-    return (blk(e) / blk(r).clamp(min=1e-6)).max().item()
-
-
 def make_case(CK, TK, layout, M, N, Kd, epi, odt, seed):
-    """(run: () -> outputs, oracle outputs in fp32).  run() returns a tuple of the tensors the GEMM wrote."""
+    """(run: () -> outputs, keyword arguments of GR.gemm_ratios).  run() returns a tuple of the tensors the GEMM
+    wrote."""
     g = torch.Generator(device=DEV).manual_seed(seed)
     rnd = lambda *s, scale=1.0: (torch.randn(*s, generator=g, device=DEV) * scale).bfloat16()
     if epi == "swiglu":
         Fh = N // 2
         x, w = rnd(M, Kd, scale=0.5), rnd(N, Kd, scale=Kd ** -0.5)
-        gu0 = x.float() @ w.float().t()
 
         def run():   # the launcher itself, so that an F the wide tile cannot take reaches it
             gu = torch.empty(M, N, dtype=torch.bfloat16, device=DEV)
             act = torch.empty(M, Fh, dtype=torch.bfloat16, device=DEV)
             CK._C.gemm(x, w, gu, 0, 5, None, aux=act, swiglu_F=Fh, gate_first=True)
             return gu, act
-        return run, (gu0, None)
+        return run, dict(a=x, b=w, layout="nt", epi="swiglu")
     if epi == "swiglu_bwd":
         dy, w2, gu = rnd(M, Kd, scale=0.5), rnd(Kd, N, scale=Kd ** -0.5), rnd(M, 2 * N)
-        ref = TK.swiglu_bwd(dy.float() @ w2.float(), gu.float())
-        return (lambda: (CK.gated_down_bwd(dy, w2, gu),)), (ref,)
+        return (lambda: (CK.gated_down_bwd(dy, w2, gu),)), dict(a=dy, b=w2, layout="nn", epi="swiglu_bwd", aux=gu)
     a = rnd(*((M, Kd) if layout != "tn" else (Kd, M)), scale=0.5)
     b = rnd(*((N, Kd) if layout == "nt" else (Kd, N)), scale=Kd ** -0.5)
-    ref = TK.gemm(a.float(), b.float(), layout)
+    ref = dict(a=a, b=b, layout=layout, epi=epi)
     if epi == "rope":
         hd, kvh = (HD, KVH) if N == QKV else (64, 2)
         h = N // hd - 2 * kvh
         ang = torch.arange(M, device=DEV, dtype=torch.float32)[:, None] * (1e4 ** (-torch.arange(0, hd, 2, device=DEV) / hd))
         table = torch.stack((ang.cos(), ang.sin()), -1).contiguous()
         Sr = min(M, S)
-        ref = TK.gemm(a.float(), b.float(), layout, rope=(table, Sr, hd, h, kvh))
-        return (lambda: (CK.gemm(a, b, layout, rope=(table, Sr, hd, h, kvh)),)), (ref,)
+        ref.update(rope=(table, Sr, hd, (h + kvh) * hd))
+        return (lambda: (CK.gemm(a, b, layout, rope=(table, Sr, hd, h, kvh)),)), ref
     if epi == "residual":
         r = rnd(M, N)
-        return (lambda: (CK.gemm(a, b, layout, residual=r),)), (ref + r.float(),)
+        return (lambda: (CK.gemm(a, b, layout, residual=r),)), dict(ref, extra=r)
     if epi == "accumulate":
         c0 = rnd(M, N).to(odt)
 
@@ -113,14 +103,14 @@ def make_case(CK, TK, layout, M, N, Kd, epi, odt, seed):
             c = c0.clone()
             CK.gemm(a, b, layout, out=c, accumulate=True)
             return (c,)
-        return run, (ref + c0.float(),)
-    return (lambda: (CK.gemm(a, b, layout, out_dtype=odt),)), (ref,)
+        return run, dict(ref, extra=c0)
+    return (lambda: (CK.gemm(a, b, layout, out_dtype=odt),)), ref
 
 
 def check(K, case):
     CK, TK = K
     name, layout, M, N, Kd, epi, odt = case
-    run, refs = make_case(CK, TK, layout, M, N, Kd, epi, odt, seed=sum(map(ord, name)))
+    run, ref = make_case(CK, TK, layout, M, N, Kd, epi, odt, seed=sum(map(ord, name)))
     outs = {}
     for mode in ("wide", "narrow"):
         with tile(CK, mode):
@@ -128,11 +118,11 @@ def check(K, case):
             outs[mode] = run()
             torch.cuda.synchronize()
             assert CK.launch_count() == n0 + 1, "one launch of our kernel per GEMM"
-    if epi == "swiglu":   # the activation of the bf16-rounded projection, as both kernels compute it
-        refs = (refs[0], TK.swiglu_fwd(outs["narrow"][0].float()))
+    for mode in ("wide", "narrow"):
+        r = GR.gemm_ratios(list(outs[mode]), **ref)
+        assert all(v <= 1.0 for v in r), (name, mode, r)
     worst = 0.0
-    for w, n, ref in zip(outs["wide"], outs["narrow"], refs):
-        assert tile_rel(w, ref) < 1e-2, name
+    for w, n in zip(outs["wide"], outs["narrow"]):
         d = (w.float() - n.float()).abs()
         worst = max(worst, d.max().item())
         # the same per-element k order: equal up to the last bit of the output type

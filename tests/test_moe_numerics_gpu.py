@@ -290,36 +290,3 @@ def test_moe_mlp_node(CK, shape, regime):
         J("z", "scalar", MR.scalar_ratio(z, ref["z"]))
         del ref, y, dh, dwr, dw1, dw2
         J.done(enforce=path == "cuda")
-
-
-# ------------------------------------------------------------------------------------ dense fp32 outputs
-# (name, layout, M, N, K, accumulate): the fp32-output cases of test_gemm_wide_gpu.py / test_gemm_epilogue_gpu.py and
-# the router-logit GEMM of Qwen3-30B-A3B
-DENSE_FP32 = [
-    ("fp32_store", "nn", 640, 1288, 256, False),
-    ("fp32_accum", "tn", 1000, 520, 200, True),
-    ("head_dw_fp32", "tn", 32000, 2048, 4096, True),
-    ("router_logits", "nt", 8192, 128, 2048, False),
-]
-
-
-@pytest.mark.parametrize("case", DENSE_FP32, ids=lambda c: c[0])
-@pytest.mark.parametrize("tile", [0, 1, 2], ids=["auto", "narrow", "wide"])
-def test_dense_fp32_outputs(CK, case, tile):
-    name, layout, M, N, Kd, acc = case
-    g = torch.Generator(device=DEV).manual_seed(9)
-    a = rnd(g, *((M, Kd) if layout != "tn" else (Kd, M)))
-    b = rnd(g, *((N, Kd) if layout == "nt" else (Kd, N)))
-    base = torch.randn(M, N, generator=g, device=DEV)
-    out = base.clone() if acc else torch.empty(M, N, device=DEV)
-    CK._C._set_gemm_tile(tile)
-    try:
-        CK.gemm(a, b, layout, out=out, accumulate=acc)
-    finally:
-        CK._C._set_gemm_tile(0)
-    A = a.to(F64).t() if layout == "tn" else a.to(F64)
-    B = b.to(F64).t() if layout == "nt" else b.to(F64)
-    ref = A @ B + (base.to(F64) if acc else 0)
-    J = Judge(f"dense fp32 {name} tile {tile}")
-    J(name, "fp32", MR.ratio(out, ref))
-    J.done()
