@@ -1,7 +1,7 @@
-"""Attention kernels, causal, hd 128: the pipelined kernels (what the model runs) against the lock-step kernels they
-replaced and the library (cuDNN / flash SDPA through torch), forward and backward, in alternated rounds; plus numerics
-vs the fp32 oracle at a small shape.  Shapes: the Llama2-1.4B headline block (B2 H16 KVH4 S4096), B2 H32 S4096, and both
-with 512-token documents.  Prints the card, its power limit and the SM clock from the same run.
+"""Attention kernels, causal, hd 128: the pipelined kernels (what the model runs) against the library (cuDNN / flash
+SDPA through torch), forward and backward, in alternated rounds; plus numerics vs the fp32 oracle at a small shape.
+Shapes: the Llama2-1.4B headline block (B2 H16 KVH4 S4096), B2 H32 S4096, and both with 512-token documents.  Prints
+the card, its power limit and the SM clock from the same run.
 
     python scripts/attn_bench.py [--rounds 5] [--dump DIR]
 
@@ -98,17 +98,12 @@ for name, H, KVH, L in SHAPES:
     fl = 4 * H * pairs * hd                 # useful forward FLOPs: 2 GEMMs over the visible pairs
     o, l = C.attn_fwd(qkv, B, S, H, KVH, hd, sc, seg)
     dq = C.attn_bwd(do, qkv, o, l, B, S, H, KVH, hd, sc, None, seg)
-    o_r, l_r = C.attn_fwd_lockstep(qkv, B, S, H, KVH, hd, sc, seg)
-    dq_r = C.attn_bwd_lockstep(do, qkv, o_r, l_r, B, S, H, KVH, hd, sc, None, seg)
-    same = dict(o=torch.equal(o, o_r), lse=torch.equal(l, l_r), dqkv=torch.equal(dq, dq_r))
     if a.dump and L is None:
         os.makedirs(a.dump, exist_ok=True)
         torch.save(dict(o=o.cpu(), lse=l.cpu(), dqkv=dq.cpu()), os.path.join(a.dump, f"{name}.pt"))
     arms = {
         "pipelined": (lambda: C.attn_fwd(qkv, B, S, H, KVH, hd, sc, seg),
                       lambda: C.attn_bwd(do, qkv, o, l, B, S, H, KVH, hd, sc, None, seg)),
-        "lockstep": (lambda: C.attn_fwd_lockstep(qkv, B, S, H, KVH, hd, sc, seg),
-                     lambda: C.attn_bwd_lockstep(do, qkv, o, l, B, S, H, KVH, hd, sc, None, seg)),
     }
     if L is None:                           # the library bar (causal only)
         q = qkv[:, :H * hd].reshape(B, S, H, hd).transpose(1, 2).contiguous().requires_grad_()
@@ -148,7 +143,6 @@ for name, H, KVH, L in SHAPES:
         out.append(dict(kind="time", shape=name, arm=arm, fwd_ms=statistics.median(tf), fwd_min=min(tf), fwd_max=max(tf),
                         bwd_ms=statistics.median(tb), bwd_min=min(tb), bwd_max=max(tb),
                         fwd_tflops=fl / statistics.median(tf) / 1e9, bwd_tflops=2.5 * fl / statistics.median(tb) / 1e9))
-    out.append(dict(kind="bitwise_vs_lockstep", shape=name, **same))
     del arms
     torch.cuda.empty_cache()
 

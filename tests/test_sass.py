@@ -74,8 +74,8 @@ def test_no_legacy_warp_level_mma_anywhere(kernels):
 def test_hot_kernels_use_wgmma_and_tma(kernels):
     gemm = _has(kernels, "gemm_bf16_wgmma", r"HGMMA\.64x128x16|QGMMA\.64x128x32", r"UTMALDG\.[24]D", r"WARPGROUP\.ARRIVE")
     assert len(gemm) >= 20
-    _has(kernels, "attn_fwd_kernel", r"HGMMA\.64x128x16", r"UTMALDG", r"MUFU\.EX2")
-    _has(kernels, "attn_bwd_kernel", r"HGMMA\.64x64x16", r"UTMALDG", r"MUFU\.EX2")
+    _has(kernels, "attn_fwd_pipe_kernel", r"HGMMA\.64x128x16", r"UTMALDG", r"MUFU\.EX2")
+    _has(kernels, "attn_bwd_pipe_kernel", r"HGMMA\.64x64x16", r"UTMALDG", r"MUFU\.EX2")
     # fp8 instantiation: e4m3 warpgroup MMA
     assert any("QGMMA.64x128x32.F32.E4M3.E4M3" in b for k, b in kernels.items() if "gemm_bf16_wgmma" in k)
 
