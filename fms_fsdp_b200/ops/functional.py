@@ -164,12 +164,7 @@ class _RMSNorm(torch.autograd.Function):
         dx, dw32 = K.rmsnorm_bwd(dy.reshape(-1, D).contiguous(), x.reshape(-1, D), _wdata(w), rstd)
         dw = None
         if ctx.needs_input_grad[1]:
-            def put(out, acc):
-                if acc:
-                    out.add_(dw32.to(out.dtype))
-                else:
-                    out.copy_(dw32)
-            dw = _deliver_wgrad(w, put)
+            dw = _deliver_wgrad(w, _put_fp32(dw32))
         return dx.view_as(x), dw, None
 
 
@@ -200,12 +195,7 @@ class _RMSNormFork(torch.autograd.Function):
                                  None if dres is None else dres.reshape(-1, D))
         dw = None
         if ctx.needs_input_grad[1]:
-            def put(out, acc):
-                if acc:
-                    out.add_(dw32.to(out.dtype))
-                else:
-                    out.copy_(dw32)
-            dw = _deliver_wgrad(w, put)
+            dw = _deliver_wgrad(w, _put_fp32(dw32))
         return dx.view_as(x), dw, None
 
 
@@ -341,9 +331,11 @@ class _QKVAttention(torch.autograd.Function):
 
 
 def _put_fp32(val):
+    """Delivery of an fp32 gradient ``val``: stored, or added to the slot in fp32 and rounded once to the slot's dtype
+    (rounding ``val`` to a bf16 slot's dtype before the add would round twice)."""
     def put(out, acc):
         if acc:
-            out.add_(val.to(out.dtype))
+            out.copy_(out.to(val.dtype) + val)
         else:
             out.copy_(val)
     return put

@@ -108,7 +108,7 @@ class ShardUnit:
             buf = p._grad_buf
             if p.grad is not None:
                 if p._grad_ready:
-                    buf.add_(p.grad.to(buf.dtype).view_as(buf))
+                    buf.copy_(buf + p.grad.view_as(buf))     # in the wider dtype, rounded once
                 else:
                     buf.copy_(p.grad.view_as(buf))
                 p._grad_ready = True
