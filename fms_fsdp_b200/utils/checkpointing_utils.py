@@ -256,7 +256,8 @@ class Checkpointer:
         t0 = time.time()
 
         if os.path.isfile(load_path):
-            ckp = torch.load(load_path, map_location="cpu", weights_only=False)
+            # memory-mapped: the ranks of a node share the file's page cache instead of each holding a copy
+            ckp = torch.load(load_path, map_location="cpu", weights_only=False, mmap=True)
             sd = ckp.get("model_state", ckp)
             sd = sd.get("_orig_mod", sd) if isinstance(sd, dict) and "_orig_mod" in sd else sd
             eng.load_full_state_dict(sd, strict=strict)

@@ -1,5 +1,6 @@
 """Export a sharded training checkpoint to a HuggingFace ``LlamaForCausalLM`` directory (``Qwen3ForCausalLM`` for variants
-with QK-norm, ``Qwen2ForCausalLM`` for variants with q / k / v biases)
+with QK-norm, ``Qwen2ForCausalLM`` for variants with q / k / v biases, ``Qwen3MoeForCausalLM`` / ``MixtralForCausalLM``
+for mixture-of-experts variants with / without QK-norm)
 (CLI parity with reference ``fms_to_hf_llama.py:133-171``):
 
     python fms_to_hf_llama.py --model_variant llama2_7b --nocompiled --load_path <step_N_ckp> \
@@ -38,10 +39,18 @@ def _interleaved_to_halfsplit_bias(b: torch.Tensor, nheads: int) -> torch.Tensor
 def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
     """``is_old_fms`` is kept for the reference's signature; this repo's LLaMA is always fused, pre-fusion checkpoints are
     fused when they are read (``load_dcp_into``).  A model with ``qk_norm`` is written as a ``Qwen3ForCausalLM``, one with
-    ``qkv_bias`` as a ``Qwen2ForCausalLM`` (both with an untied head), every other one as a ``LlamaForCausalLM``."""
+    ``qkv_bias`` as a ``Qwen2ForCausalLM`` (both with an untied head), every other one as a ``LlamaForCausalLM``.
+    Mixture-of-experts models (``moe_num_experts > 0``) are written as a ``Qwen3MoeForCausalLM`` with ``qk_norm`` and a
+    ``MixtralForCausalLM`` without; ``save_pretrained`` stores their experts in the per-expert hub layout."""
     from transformers import LlamaConfig, LlamaForCausalLM
 
     c = model.config
+    moe = c.moe_num_experts > 0
+    if moe and getattr(c, "qkv_bias", False):
+        raise NotImplementedError("a mixture-of-experts model with q / k / v biases has no HF class to export to")
+    if moe and not c.qk_norm and not c.moe_norm_topk:
+        raise NotImplementedError("Mixtral renormalises the top-k router weights; a mixture-of-experts model without "
+                                  "QK-norm and with moe_norm_topk=False has no HF class to export to")
     rope_theta = c.rope_theta
     if c.ntk_scaling:
         alpha = model.rot_emb._alpha(c.max_expected_seq_len)
@@ -58,7 +67,21 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
         kw["rope_scaling"] = dict(c.rope_scaling)
     if getattr(c, "attn_head_dim", None):
         kw["head_dim"] = c.head_dim
-    if getattr(c, "qk_norm", False):
+    if moe:
+        kw.pop("mlp_bias")
+        kw.update(num_experts_per_tok=c.moe_top_k, router_aux_loss_coef=c.moe_aux_loss_coef)
+    if moe and c.qk_norm:
+        from transformers import Qwen3MoeConfig, Qwen3MoeForCausalLM
+        kw["head_dim"] = c.head_dim
+        hf = Qwen3MoeForCausalLM(Qwen3MoeConfig(**kw, num_experts=c.moe_num_experts, moe_intermediate_size=c.moe_hidden_dim,
+                                                norm_topk_prob=c.moe_norm_topk, decoder_sparse_step=1, mlp_only_layers=[],
+                                                use_sliding_window=False))
+    elif moe:
+        from transformers import MixtralConfig, MixtralForCausalLM
+        kw.pop("attention_bias")
+        kw["intermediate_size"] = c.moe_hidden_dim
+        hf = MixtralForCausalLM(MixtralConfig(**kw, num_local_experts=c.moe_num_experts, sliding_window=None))
+    elif getattr(c, "qk_norm", False):
         from transformers import Qwen3Config, Qwen3ForCausalLM
         kw.pop("mlp_bias")
         kw["head_dim"] = c.head_dim
@@ -91,11 +114,16 @@ def convert_to_hf(model: LLaMA, model_variant: str, is_old_fms: bool = False):
             if getattr(c, "qk_norm", False):
                 layer.self_attn.q_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.q_norm.weight"]))
                 layer.self_attn.k_norm.weight.copy_(_interleaved_to_halfsplit_vec(sd[p + "attn.k_norm.weight"]))
-            fused = sd[p + "ff_sub_layer.wg1_fused.weight"]
-            wg, w1 = torch.split(fused, [fused.size(0) // 2, fused.size(0) // 2], dim=0)
-            layer.mlp.gate_proj.weight.copy_(wg)
-            layer.mlp.up_proj.weight.copy_(w1)
-            layer.mlp.down_proj.weight.copy_(sd[p + "ff_sub_layer.w2.weight"])
+            if moe:          # transformers 5 holds the experts fused, in this repo's [E, 2F (gate | up), D] / [E, D, F]
+                layer.mlp.gate.weight.copy_(sd[p + "moe.gate.weight"])
+                layer.mlp.experts.gate_up_proj.copy_(sd[p + "moe.w1"])
+                layer.mlp.experts.down_proj.copy_(sd[p + "moe.w2"])
+            else:
+                fused = sd[p + "ff_sub_layer.wg1_fused.weight"]
+                wg, w1 = torch.split(fused, [fused.size(0) // 2, fused.size(0) // 2], dim=0)
+                layer.mlp.gate_proj.weight.copy_(wg)
+                layer.mlp.up_proj.weight.copy_(w1)
+                layer.mlp.down_proj.weight.copy_(sd[p + "ff_sub_layer.w2.weight"])
             layer.input_layernorm.weight.copy_(sd[p + "ln.weight"])
             layer.post_attention_layernorm.weight.copy_(sd[p + "ff_ln.weight"])
         hf.model.norm.weight.copy_(sd["dec_norm.weight"])
