@@ -24,6 +24,7 @@ import torch.nn.functional as F
 
 from fms_fsdp_b200 import ops
 from fms_fsdp_b200.ops import torch_kernels
+from fms_fsdp_b200.ops.functional import _deliver_wgrad, _put_fp32
 
 CausalLMOutput = namedtuple("CausalLMOutput", ["logits"])
 
@@ -152,7 +153,7 @@ class Mamba2(nn.Module):
         B, S, _ = u.shape
         zxbcdt = self.in_proj(u).view(B * S, -1)
         z, xBC, dt = torch.split(zxbcdt, [self.d_inner, self.conv_dim, self.nheads], dim=-1)
-        xBC = ops.causal_conv1d(xBC.contiguous(), _conv_w(self.conv1d), self.conv1d.bias, S, True)
+        xBC = ops.causal_conv1d(xBC.contiguous(), self.conv1d.weight, self.conv1d.bias, S, True)
         x, Bm, Cm = torch.split(xBC, [self.d_inner, self.ngroups * self.d_state, self.ngroups * self.d_state], dim=-1)
         y = ops.ssd_scan(x.reshape(B * S, self.nheads, self.headdim), dt.contiguous(), _neg_exp(self.A_log),
                          Bm.reshape(B * S, self.ngroups, self.d_state), Cm.reshape(B * S, self.ngroups, self.d_state),
@@ -178,45 +179,7 @@ class _NegExp(torch.autograd.Function):
     def backward(ctx, dA):
         (a,) = ctx.saved_tensors
         g = dA * a  # d(-exp(x))/dx = -exp(x) = a
-        p = ctx.param
-        buf = getattr(p, "_grad_buf", None)
-        if buf is not None:
-            if getattr(p, "_grad_ready", False):
-                buf.add_(g.to(buf.dtype))
-            else:
-                buf.copy_(g)
-            p._grad_ready = True
-            return None
-        return g.to(p.dtype)
-
-
-class _ConvW(torch.autograd.Function):
-    """[C,1,K] parameter viewed as [C,K] without creating an autograd-saved view of the gathered buffer."""
-
-    @staticmethod
-    def forward(ctx, w):
-        ctx.param = w
-        data = w.data if isinstance(w, nn.Parameter) else w
-        # a private copy (C x K, tiny): the gathered buffer it came from is recycled before backward
-        return data.reshape(data.shape[0], data.shape[-1]).clone()
-
-    @staticmethod
-    def backward(ctx, g):
-        p = ctx.param
-        buf = getattr(p, "_grad_buf", None)
-        if buf is not None:
-            gv = g.reshape(buf.shape)
-            if getattr(p, "_grad_ready", False):
-                buf.add_(gv.to(buf.dtype))
-            else:
-                buf.copy_(gv)
-            p._grad_ready = True
-            return None
-        return g.reshape(p.shape).to(p.dtype)
-
-
-def _conv_w(conv: _Conv1dParams):
-    return _ConvW.apply(conv.weight)
+        return _deliver_wgrad(ctx.param, _put_fp32(g))
 
 
 class _WB(nn.Module):
@@ -265,7 +228,7 @@ class Mamba1(nn.Module):
     def forward(self, u):
         B, S, _ = u.shape
         x, z = self.in_proj(u).view(B * S, -1).chunk(2, dim=-1)
-        x = ops.causal_conv1d(x.contiguous(), _conv_w(self.conv1d), self.conv1d.bias, S, True)
+        x = ops.causal_conv1d(x.contiguous(), self.conv1d.weight, self.conv1d.bias, S, True)
         dt, Bm, Cm = torch.split(ops.linear(x, self.x_proj.weight), [self.dt_rank, self.d_state, self.d_state], dim=-1)
         delta = ops.linear(dt.contiguous(), self.dt_proj.weight)
         y = ops.selective_scan(x, delta, _neg_exp(self.A_log), Bm.contiguous(), Cm.contiguous(), self.D, z.contiguous(),

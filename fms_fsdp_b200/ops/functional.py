@@ -217,12 +217,7 @@ class _RMSNormGated(torch.autograd.Function):
     def backward(ctx, dy):
         x, z, rstd = ctx.saved_tensors
         dx, dz, dw32 = ctx.K.rmsnorm_gated_bwd(dy.contiguous(), x, z, _wdata(ctx.w), rstd, ctx.gs)
-        def put(out, acc):
-            if acc:
-                out.add_(dw32.to(out.dtype))
-            else:
-                out.copy_(dw32)
-        dw = _deliver_wgrad(ctx.w, put) if ctx.needs_input_grad[2] else None
+        dw = _deliver_wgrad(ctx.w, _put_fp32(dw32)) if ctx.needs_input_grad[2] else None
         return dx, dz, dw, None, None
 
 
@@ -599,12 +594,7 @@ class _AddRMSNorm(torch.autograd.Function):
         dres = dn.float()
         if dres_out is not None:
             dres = dres + dres_out.reshape(-1, D).float()
-        def put(out, acc):
-            if acc:
-                out.add_(dw32.to(out.dtype))
-            else:
-                out.copy_(dw32)
-        dw = _deliver_wgrad(ctx.w, put) if ctx.needs_input_grad[2] else None
+        dw = _deliver_wgrad(ctx.w, _put_fp32(dw32)) if ctx.needs_input_grad[2] else None
         return dres.to(ctx.xdtype).view(dy.shape), dres.to(res_out.dtype).view(dy.shape), dw, None, None
 
 
@@ -762,34 +752,34 @@ def cross_entropy_z(logits, labels, z_loss_coef, ignore_index=-100):
 
 
 # ------------------------------------------------------------------------------------------- mamba
+def _conv_taps(w):
+    """The [C, K] taps of a depthwise conv weight, given as [C, K] or in nn.Conv1d's [C, 1, K] shape."""
+    wd = _wdata(w)
+    return wd.reshape(wd.shape[0], wd.shape[-1])
+
+
 class _CausalConv1d(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w, b, seq_len, activation):
         K = kernels_for(x)
         ctx.K, ctx.w, ctx.b, ctx.args = K, w, b, (seq_len, activation)
         ctx.save_for_backward(x)
-        return K.causal_conv1d_fwd(x, _wdata(w), None if b is None else _wdata(b), seq_len, activation)
+        return K.causal_conv1d_fwd(x, _conv_taps(w), None if b is None else _wdata(b), seq_len, activation)
 
     @staticmethod
     def backward(ctx, dy):
         (x,) = ctx.saved_tensors
         seq_len, activation = ctx.args
         w, b = ctx.w, ctx.b
-        dx, dw32, db32 = ctx.K.causal_conv1d_bwd(dy.contiguous(), x, _wdata(w),
+        dx, dw32, db32 = ctx.K.causal_conv1d_bwd(dy.contiguous(), x, _conv_taps(w),
                                                  None if b is None else _wdata(b), seq_len, activation)
-        def putter(val):
-            def put(out, acc):
-                if acc:
-                    out.add_(val.to(out.dtype))
-                else:
-                    out.copy_(val)
-            return put
-        dw = _deliver_wgrad(w, putter(dw32))
-        db = None if b is None else _deliver_wgrad(b, putter(db32))
+        dw = _deliver_wgrad(w, _put_fp32(dw32.view(w.shape)))
+        db = None if b is None else _deliver_wgrad(b, _put_fp32(db32))
         return dx, dw, db, None, None
 
 
 def causal_conv1d(x, w, b, seq_len, activation=True):
+    """Depthwise causal conv1d (+ SiLU) of x [B*S, C] restarting at every sequence; w [C, K] or [C, 1, K]."""
     return _CausalConv1d.apply(x, w, b, seq_len, activation)
 
 
@@ -830,16 +820,9 @@ class _SSDScan(torch.autograd.Function):
             rest = gs[5:]
             dD = rest.pop(0) if D is not None else None
             ddtb = rest.pop(0) if dt_bias is not None else None
-        def putter(val):
-            def put(out, acc):
-                if acc:
-                    out.add_(val.to(out.dtype))
-                else:
-                    out.copy_(val)
-            return put
-        gA = _deliver_wgrad(A, putter(dA))
-        gD = None if D is None else _deliver_wgrad(D, putter(dD))
-        gb = None if dt_bias is None else _deliver_wgrad(dt_bias, putter(ddtb))
+        gA = _deliver_wgrad(A, _put_fp32(dA))
+        gD = None if D is None else _deliver_wgrad(D, _put_fp32(dD))
+        gb = None if dt_bias is None else _deliver_wgrad(dt_bias, _put_fp32(ddtb))
         return (dx.to(x.dtype), ddt.to(dt.dtype), gA, dB.to(Bm.dtype), dC.to(Cm.dtype), gD, gb, None, None)
 
 
@@ -881,16 +864,9 @@ class _SelectiveScan(torch.autograd.Function):
             dD = rest.pop(0) if D is not None else None
             dz = rest.pop(0) if z is not None else None
             ddb = rest.pop(0) if delta_bias is not None else None
-        def putter(val):
-            def put(out, acc):
-                if acc:
-                    out.add_(val.to(out.dtype))
-                else:
-                    out.copy_(val)
-            return put
-        gA = _deliver_wgrad(A, putter(dA))
-        gD = None if D is None else _deliver_wgrad(D, putter(dD))
-        gb = None if delta_bias is None else _deliver_wgrad(delta_bias, putter(ddb))
+        gA = _deliver_wgrad(A, _put_fp32(dA))
+        gD = None if D is None else _deliver_wgrad(D, _put_fp32(dD))
+        gb = None if delta_bias is None else _deliver_wgrad(delta_bias, _put_fp32(ddb))
         return (du.to(u.dtype), dd.to(delta.dtype), gA, dB.to(Bm.dtype), dC.to(Cm.dtype), gD,
                 None if z is None else dz.to(z.dtype), gb, None)
 

@@ -483,14 +483,17 @@ def run_node(call, acts, weights, dos, mode):
             out = call()
             outs = out if isinstance(out, tuple) else (out,)
             first = outs if first is None else first
-            names = list(acts) + (list(weights) if mode == "returned" else [])
-            leaves = [acts[n] for n in acts] + ([weights[n] for n in weights] if mode == "returned" else [])
-            gr = torch.autograd.grad(outs, leaves, do if isinstance(do, tuple) else (do,), allow_unused=True)
-            got = dict(zip(names, gr))
-            for n in acts:
-                dacts[n] = got[n] if n not in dacts else dacts[n] + got[n]
-            after.append({n: (got[n] if mode == "returned" else p._grad_buf.clone()) for n, p in weights.items()})
+            # a whole backward, as the engine runs it: ``autograd.grad`` would skip the nodes that lead only to
+            # parameters (``_NegExp`` of Mamba's A_log), whose gradients are delivered as a side effect
+            for t in list(acts.values()) + list(weights.values()):
+                t.grad = None
+            torch.autograd.backward(outs, do if isinstance(do, tuple) else (do,))
+            for n, a in acts.items():
+                dacts[n] = a.grad if n not in dacts else dacts[n] + a.grad
+            after.append({n: (p.grad if mode == "returned" else p._grad_buf.clone()) for n, p in weights.items()})
     finally:
+        for t in list(acts.values()) + list(weights.values()):
+            t.grad = None
         for p in weights.values():
             p._grad_buf, p._grad_ready = None, False
     return first, dacts, after
